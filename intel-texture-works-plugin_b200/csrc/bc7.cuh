@@ -5,10 +5,13 @@
 // that reuse the per-group scratch; the chain phase -- 14 to 18 roles per block, a quarter of the work -- runs ONCE for all
 // sixteen blocks, two lanes per block, so that a pass is two equally long roles wide (DESIGN.md section 4 has the numbers).
 // The 32 lanes are spread over the blocks' independent work items instead of over texels:
-//   * shape phases: lane <-> (block slot, partition shape).  A lane fits the PCA segments of its
-//     shape ONCE and evaluates both BC7 modes that use that shape (0 and 2 share the three-subset
-//     shapes, 1 and 3 the two-subset shapes; the reference refits per mode, K:1279-1297, with
-//     identical results because the fit does not depend on the mode);
+//   * shape phases: a shape's error is the sum of its subsets' errors, and a subset's fit, endpoints and error depend on its
+//     texel mask alone (the reference refits per shape and mode, K:1279-1297, with identical results).  So the three-subset
+//     shapes go lane <-> (block, distinct mask): fit once, quantise for modes 0 and 2 and search for mode 2, then lane <->
+//     (block, shape) adds three stored mode-2 errors and searches mode 0 from the stored endpoints.  The two-subset shapes
+//     (modes 1, 3) go lane <-> mask per block when the profile searches all 64 of them (the split keys then come from the
+//     fits' power iterations); for shorter lists and for mode 7 a lane evaluates one ranked shape: it fits each subset once
+//     and searches it for both modes of the pair;
 //   * ranking phase: lane <-> (block slot, two-subset shape) for the 64 PCA split bounds;
 //   * chain phase: lane <-> (block slot, role).  The per-mode refinement chains, the mode 4/5
 //     rotation / index-swap candidates and mode 6 are independent of one another in the reference
@@ -37,6 +40,7 @@
 // functions lane by lane on the CPU (test-only).
 #pragma once
 #include "bc67_core.cuh"
+#include "itw_masks2.cuh"
 #include "itw_masks3.cuh"
 
 // unroll factors of the two hottest loops; on H100 (tools/tune_unroll.sh) BC7 slow / basic take 33.65 / 13.51 ms at
@@ -53,6 +57,8 @@ namespace itw {
 // distinct subset masks of the three-subset shapes and the mask ids of each shape (tools/gen_mask_tables.py)
 ITW_TABLE_DECL(uint16_t, mask3_unique, ITW_MASK3_COUNT)
 ITW_TABLE_DECL(uint8_t, shape3_mask_id, 64 * 3)
+// the 128 subset masks of the two-subset shapes as shape + 64 * subset, ascending popcount (tools/gen_mask_tables.py)
+ITW_TABLE_DECL(uint8_t, mask2_order, 128)
 
 // bc7_enc_settings (ispc_texcomp.h:27-41) flattened to ints for the device
 struct Bc7Params {
@@ -80,9 +86,8 @@ struct Bc7Warp {
     Bc7Block blk[kBc7Batch];                   // the half the shape phases are working on
     union {
         // per-GROUP scratch (slot = block index inside the group), reused by every group in turn
-        int cand_err[kBc7Slots][2][64];        // errors of the mode-slot pair being evaluated: [first/second][list position]
-        int keys[kBc7Slots][64];               // split-bound keys of the set being ranked: dead once `order` is written, and
-                                               // the candidate errors of the previous pair have been consumed by then
+        int cand_err[kBc7Slots][2][64];        // errors of the mode-slot pair being evaluated: [first/second][list position,
+                                               // or shape id on the full two-subset path (bc7_full_two)]
         // end of the chain phase -> store phase (the shape phases are over by then)
         struct {
             int err[32], role[32];             // best (error, role) of the roles a lane ran for ITS block ...
@@ -94,12 +99,20 @@ struct Bc7Warp {
     u32 palette[40][32];                       // lane-private scratch of the index search, [entry][lane]: 24 palette
                                                // entries, then 5 per-subset constants x 3 subsets
     union {
-        // decoded endpoints (A, B as RGBA bytes) of every DISTINCT three-subset mask, for the two blocks being processed:
-        // mode 2 for all 140 masks, mode 0 for the 36 masks of shapes 0..15 (bc7_phase_masks3 -> bc7_phase_shapes3)
+        // every DISTINCT three-subset mask, for the two blocks being processed (bc7_phase_masks3 -> bc7_phase_shapes3): the
+        // mode-2 subset error of all 140 masks, the decoded mode-0 endpoints (A, B as RGBA bytes) of the 36 masks of shapes 0..15
         struct {
-            u32 mode2[2][ITW_MASK3_COUNT][2];
-            u32 mode0[2][ITW_MASK3_FIRST][2];
-        } ends3;
+            int err2[2][ITW_MASK3_COUNT];
+            u32 ends0[2][ITW_MASK3_FIRST][2];
+        } masks3;
+        // two-subset shapes of the group, after its three-subset phases
+        struct {
+            int keys[kBc7Slots][64];           // split-bound keys of the set being ranked: dead once `order` is written
+            // full lists (bc7_full_two), one block at a time: mode 1 / mode 3 errors and split bounds of the 128 subset
+            // masks, [shape + 64 * subset] (bc7_phase_masks2 -> bc7_phase_shapes2)
+            int mode1[128], mode3[128];
+            float bound[128];
+        } two;
         // chain phase of a two-half round: the FIRST half again (re-read from the staged tile once its slot in blk[] has
         // been taken by the second half; the mask tables are dead by then)
         Bc7Block parked[kBc7Batch];
@@ -197,12 +210,15 @@ ITW_HD void load_planes(u32 (&P)[4][4], const View& v)
         for (int i = 0; i < 4; i++) P[c][i] = view_plane(v, c, i);
 }
 
-// Power iteration on a packed symmetric matrix [xx xy xz xw yy yz yw zz zw ww]; K:207-229.  Unroll factor measured
-// (tools/tune_unroll.sh): rolled by 4 in round 1, when the kernel was instruction-cache bound; fully unrolled is 0.4 % faster now.
+// Power iteration on a packed symmetric matrix [xx xy xz xw yy yz yw zz zw ww]; K:207-229.  Continues from the vector in
+// `axis` (the reference starts from (1, 1, 1, 1)); kIterations is even, so the renormalisation keeps the reference's parity
+// when a run is split in two.  Unroll factor measured (tools/tune_unroll.sh): rolled by 4 in round 1, when the kernel was
+// instruction-cache bound; fully unrolled is 0.4 % faster now.
 template <int CH, int kIterations>
 ITW_HD void bc7_power_axis(float (&axis)[4], const float (&m)[10])
 {
-    float v0 = 1.0f, v1 = 1.0f, v2 = 1.0f, v3 = 1.0f;
+    static_assert(kIterations % 2 == 0, "renormalisation parity");
+    float v0 = axis[0], v1 = axis[1], v2 = axis[2], v3 = axis[3];
     ITW_UNROLL(ITW_BC7_POWER_UNROLL)
     for (int it = 0; it < kIterations; it++) {
         float a0, a1, a2, a3 = 0.0f;
@@ -260,21 +276,50 @@ struct Bc7Seg { float v[8]; };                       // endpoints A (r,g,b,a) an
 struct Bc7Packed { u32 dec_a, dec_b, q_a, q_b; };    // decoded A, B and quantised A, B as RGBA bytes
 struct Bc7Search { int err; u32 idx0, idx1; };
 
+// trace - lambda_max of a scaled covariance, from the axis of its power iteration; K:925-938
 template <int CH>
-ITW_HD void bc7_fit_impl(float (&ep)[8], const View& v, u32 mask)
+ITW_HD float bc7_bound_from_axis(const float (&cov)[10], const float (&axis)[4])
 {
+    float mv[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+    if (CH == 3) {
+        mv[0] = cov[0] * axis[0] + cov[1] * axis[1] + cov[2] * axis[2];
+        mv[1] = cov[1] * axis[0] + cov[4] * axis[1] + cov[5] * axis[2];
+        mv[2] = cov[2] * axis[0] + cov[5] * axis[1] + cov[7] * axis[2];
+    } else {
+        mv[0] = cov[0] * axis[0] + cov[1] * axis[1] + cov[2] * axis[2] + cov[3] * axis[3];
+        mv[1] = cov[1] * axis[0] + cov[4] * axis[1] + cov[5] * axis[2] + cov[6] * axis[3];
+        mv[2] = cov[2] * axis[0] + cov[5] * axis[1] + cov[7] * axis[2] + cov[8] * axis[3];
+        mv[3] = cov[3] * axis[0] + cov[6] * axis[1] + cov[8] * axis[2] + cov[9] * axis[3];
+    }
+    float sum = 0.0f;
+#pragma unroll
+    for (int c = 0; c < CH; c++) sum += sq(mv[c]);
+    float bound = cov[0] + cov[4] + cov[7];
+    if (CH == 4) bound += cov[9];
+    bound -= sqrtf(sum);
+    return max_sse(bound, 0.0f);
+}
+// kBound: also the split bound of the mask (bc7_residual_bound).  At three channels the fit's scaled covariance equals the
+// bound's (the eps the fit adds to slot 9 is never read), and the bound's four power iterations are the fit's first four.
+template <int CH, bool kBound>
+ITW_HD void bc7_fit_impl(float (&ep)[8], float& bound, const View& v, u32 mask)
+{
+    static_assert(!kBound || CH == 3, "the four-channel fit adds eps to slot 9, the split bound does not");
     u32 P[4][4];
     load_planes(P, v);
     int ist[15];
     moments_u8(ist, P, mask, CH);
-    float cov[10], mean[4], axis[4];
+    float cov[10], mean[4];
     bc7_covariance<CH>(cov, mean, ist);
     const float inv_var = 1.0f / (256.0f * 256.0f);
 #pragma unroll
     for (int i = 0; i < 10; i++) cov[i] *= inv_var;
     const float eps = 0.001f * 0.001f;
     cov[0] += eps; cov[4] += eps; cov[7] += eps; cov[9] += eps;
-    bc7_power_axis<CH, 8>(axis, cov);
+    float axis[4] = {1.0f, 1.0f, 1.0f, 1.0f};
+    bc7_power_axis<CH, 4>(axis, cov);
+    if (kBound) bound = bc7_bound_from_axis<CH>(cov, axis);
+    bc7_power_axis<CH, 4>(axis, cov);
 
     float lo = inf_f(), hi = -inf_f();
 #pragma unroll
@@ -306,9 +351,20 @@ ITW_HD_NOINLINE Bc7Seg bc7_fit(const Bc7Block* blk, int rot, int alpha, u32 mask
     Bc7Seg seg;
 #pragma unroll
     for (int i = 0; i < 8; i++) seg.v[i] = 0.0f;
-    if (channels == 4) bc7_fit_impl<4>(seg.v, v, mask);
-    else bc7_fit_impl<3>(seg.v, v, mask);
+    float unused;
+    if (channels == 4) bc7_fit_impl<4, false>(seg.v, unused, v, mask);
+    else bc7_fit_impl<3, false>(seg.v, unused, v, mask);
     return seg;
+}
+// The three-channel fit of a subset of an untransformed block, and the split bound of its mask
+struct Bc7FitBound { Bc7Seg seg; float bound; };
+ITW_HD_NOINLINE Bc7FitBound bc7_fit_bound(const Bc7Block* blk, u32 mask)
+{
+    Bc7FitBound f;
+#pragma unroll
+    for (int i = 0; i < 8; i++) f.seg.v[i] = 0.0f;
+    bc7_fit_impl<3, true>(f.seg.v, f.bound, View{blk, 3, 1}, mask);
+    return f;
 }
 
 // trace - lambda_max of a covariance; K:907-939 (eps on three diagonal slots only, K:918-920)
@@ -320,28 +376,19 @@ ITW_HD float bc7_residual_bound(float (&cov)[10])
     for (int i = 0; i < 10; i++) cov[i] *= inv_var;
     const float eps = 0.001f * 0.001f;
     cov[0] += eps; cov[4] += eps; cov[7] += eps;
-    float axis[4];
+    float axis[4] = {1.0f, 1.0f, 1.0f, 1.0f};
     bc7_power_axis<CH, 4>(axis, cov);
-    float mv[4] = {0.0f, 0.0f, 0.0f, 0.0f};
-    if (CH == 3) {
-        mv[0] = cov[0] * axis[0] + cov[1] * axis[1] + cov[2] * axis[2];
-        mv[1] = cov[1] * axis[0] + cov[4] * axis[1] + cov[5] * axis[2];
-        mv[2] = cov[2] * axis[0] + cov[5] * axis[1] + cov[7] * axis[2];
-    } else {
-        mv[0] = cov[0] * axis[0] + cov[1] * axis[1] + cov[2] * axis[2] + cov[3] * axis[3];
-        mv[1] = cov[1] * axis[0] + cov[4] * axis[1] + cov[5] * axis[2] + cov[6] * axis[3];
-        mv[2] = cov[2] * axis[0] + cov[5] * axis[1] + cov[7] * axis[2] + cov[8] * axis[3];
-        mv[3] = cov[3] * axis[0] + cov[6] * axis[1] + cov[8] * axis[2] + cov[9] * axis[3];
-    }
-    float sum = 0.0f;
-#pragma unroll
-    for (int c = 0; c < CH; c++) sum += sq(mv[c]);
-    float bound = cov[0] + cov[4] + cov[7];
-    if (CH == 4) bound += cov[9];
-    bound -= sqrtf(sum);
-    return max_sse(bound, 0.0f);
+    return bc7_bound_from_axis<CH>(cov, axis);
 }
-// Ranking key of a two-subset shape (K:952-971, :1403-1410); subset 1 = full - subset 0
+// Ranking key of a two-subset shape from the bounds of its subsets; K:952-971, :1403-1410
+ITW_HD int bc7_key_of(int shape, float bound0, float bound1)
+{
+    float b = 0.0f;
+    b += bound0;
+    b += bound1;
+    return shape + (int)((unsigned)cvt_x86(sqrtf(b) * 256.0f) * 64u);
+}
+// subset 1 = full - subset 0
 template <int CH>
 ITW_HD int bc7_split_key_impl(const Bc7Block* blk, int shape)
 {
@@ -356,10 +403,8 @@ ITW_HD int bc7_split_key_impl(const Bc7Block* blk, int shape)
     float c1[10], c2[10], mean[4];
     bc7_covariance<CH>(c1, mean, part);
     bc7_covariance<CH>(c2, mean, rest);
-    float b = 0.0f;
-    b += bc7_residual_bound<CH>(c1);
-    b += bc7_residual_bound<CH>(c2);
-    return shape + (int)((unsigned)cvt_x86(sqrtf(b) * 256.0f) * 64u);
+    const float b0 = bc7_residual_bound<CH>(c1);
+    return bc7_key_of(shape, b0, bc7_residual_bound<CH>(c2));
 }
 ITW_HD_NOINLINE int bc7_split_key(const Bc7Block* blk, int shape, int channels)
 {
@@ -461,6 +506,22 @@ ITW_HD_NOINLINE Bc7Packed bc7_quantise(Bc7Seg seg, int mode, int channels)
 // Only the shape phases do: there every lane of the warp searches the same mode at the same time, whereas a chain-phase
 // pass mixes two- and three-bit roles and two texel loops would run one after the other.
 constexpr int kAssignThresholds = 8;
+// Palette, K:1172: ((64 - w) a + w b + 32) >> 6 per channel, two channels per 32-bit word.  Written as (64 a + 32) + w (b - a):
+// the packed difference may borrow across the 16-bit lanes, but every lane of the SUM is the non-negative 14-bit value above,
+// so the word arithmetic is exact.  w = 0 and w = 64 give the endpoints.
+struct Bc7Lerp {
+    u32 base_rb, base_ga, d_rb, d_ga;
+    ITW_HD u32 entry(u32 w) const
+    {
+        return (((base_rb + w * d_rb) >> 6) & 0x00FF00FFu) | (((base_ga + w * d_ga) << 2) & 0xFF00FF00u);
+    }
+};
+ITW_HD Bc7Lerp bc7_lerp(u32 a, u32 b)
+{
+    const u32 m = 0x00FF00FFu;
+    const u32 a_rb = a & m, a_ga = (a >> 8) & m;
+    return Bc7Lerp{(a_rb << 6) + 0x00200020u, (a_ga << 6) + 0x00200020u, (b & m) - a_rb, ((b >> 8) & m) - a_ga};
+}
 ITW_HD_NOINLINE Bc7Search bc7_assign(u32 (*pal)[32], int lane, const Bc7Block* blk, int rot, int alpha, int bits_flags, int pairs,
                                      u32 pattern, u32 e0, u32 e1, u32 e2, u32 e3, u32 e4, u32 e5, u32 chmask)
 {
@@ -489,19 +550,10 @@ ITW_HD_NOINLINE Bc7Search bc7_assign(u32 (*pal)[32], int lane, const Bc7Block* b
             pal[24 + 5 * j + 3][lane] = float_bits(fdiv);
             pal[24 + 5 * j + 4][lane] = float_bits(1.0f / fdiv);  // inf when the endpoints coincide (-> NaN below, as 0/0)
         }
-        // Palette, K:1172: ((64 - w) a + w b + 32) >> 6 per channel, two channels per 32-bit word.  Written as
-        // (64 a + 32) + w (b - a): the packed difference may borrow across the 16-bit lanes, but every lane of the SUM is the
-        // non-negative 14-bit value above, so the word arithmetic is exact.  Entries 0 and levels-1 are the endpoints.
-        const u32 m = 0x00FF00FFu;
-        const u32 a_rb = a & m, a_ga = (a >> 8) & m;
-        const u32 base_rb = (a_rb << 6) + 0x00200020u, base_ga = (a_ga << 6) + 0x00200020u;
-        const u32 d_rb = (b & m) - a_rb, d_ga = ((b >> 8) & m) - a_ga;
+        const Bc7Lerp lerp = bc7_lerp(a, b);
         pal[j * levels][lane] = a;
         pal[j * levels + levels - 1][lane] = b;
-        for (int q = 1; q < levels - 1; q++) {
-            const u32 w = (u32)bc7_weight(bits, q);
-            pal[j * levels + q][lane] = (((base_rb + w * d_rb) >> 6) & m) | (((base_ga + w * d_ga) << 2) & 0xFF00FF00u);
-        }
+        for (int q = 1; q < levels - 1; q++) pal[j * levels + q][lane] = lerp.entry((u32)bc7_weight(bits, q));
     }
     const float flevels = (float)levels;
     int total = 0;
@@ -579,6 +631,55 @@ ITW_HD_NOINLINE Bc7Search bc7_assign(u32 (*pal)[32], int lane, const Bc7Block* b
         }
     }
     return Bc7Search{total, out0, out1};
+}
+// Error of ONE subset of a shape-phase search (three channels, untransformed block): bc7_assign's arithmetic -- the
+// integer-threshold two-bit form, the FMA-corrected quotient for three bits, VABSDIFF4 + IDP.4A errors -- over the texels of
+// `mask` only, with the subset's constants and palette in registers and no index bits.  The error of a shape is the sum of
+// the errors of its subsets (exact integers), and a subset's endpoints depend on its mask alone, so the shape phases search
+// every distinct mask once (modes 1, 2, 3).  The first-of-two choice adds min(e0, e1).
+ITW_HD_NOINLINE int bc7_subset_error(const Bc7Block* blk, u32 mask, u32 dec_a, u32 dec_b, int bits)
+{
+    const u32 a = dec_a & 0x00FFFFFFu, b = dec_b & 0x00FFFFFFu;
+    const u32 aa = dp4a_u8(a, a, 0u), ab = dp4a_u8(a, b, 0u), bb = dp4a_u8(b, b, 0u);
+    const int idiv = (int)(bb - 2u * ab + aa), cj = (int)(ab - aa);
+    const Bc7Lerp lerp = bc7_lerp(a, b);
+    // a counted loop over the set bits, unrolled so that the texel loads of several iterations are in flight at once (a
+    // rolled loop waits for each load: four warps per scheduler do not hide that latency)
+    const int n = popcount16(mask);
+    int total = 0;
+    if (bits == 2) {
+        // thresholds as in bc7_assign: q1 = 1 + (num >= t2) + (num >= t3), t2 <= t3
+        const int t2 = idiv ? (3 * idiv + 7) >> 3 : 0x7fffffff, t3 = idiv ? (5 * idiv + 7) >> 3 : 0x7fffffff;
+        const u32 p1 = lerp.entry((u32)bc7_weight(2, 1)), p2 = lerp.entry((u32)bc7_weight(2, 2));
+        u32 rest = mask;
+#pragma unroll 4
+        for (int i = 0; i < n; i++) {
+            const u32 low = rest & (0u - rest);
+            rest ^= low;
+            const u32 t = blk->rgb[popcount32(low - 1u)];
+            const int num = (int)dp4a_u8(t, b, 0u) - (int)dp4a_u8(t, a, 0u) - cj;
+            const bool ge2 = num >= t2, ge3 = num >= t3;
+            const u32 lo = ge3 ? p2 : (ge2 ? p1 : a), hi = ge3 ? b : (ge2 ? p2 : p1);      // palette entries q1 - 1, q1
+            const u32 d0 = absdiff_u8x4(lo, t), d1 = absdiff_u8x4(hi, t);
+            total += mini((int)dp4a_u8(d0, d0, 0u), (int)dp4a_u8(d1, d1, 0u));
+        }
+    } else {
+        const float fdiv = (float)idiv, rdiv = 1.0f / fdiv;
+        u32 rest = mask;
+#pragma unroll 4
+        for (int i = 0; i < n; i++) {
+            const u32 low = rest & (0u - rest);
+            rest ^= low;
+            const u32 t = blk->rgb[popcount32(low - 1u)];
+            const int num = (int)dp4a_u8(t, b, 0u) - (int)dp4a_u8(t, a, 0u) - cj;
+            const float proj = div_by_rcp((float)num, fdiv, rdiv);
+            const int q1 = clampi(trunc_i(fma_rn(proj, 8.0f, 0.5f)), 1, 7);
+            const u32 lo = lerp.entry((u32)bc7_weight(3, q1 - 1)), hi = lerp.entry((u32)bc7_weight(3, q1));
+            const u32 d0 = absdiff_u8x4(lo, t), d1 = absdiff_u8x4(hi, t);
+            total += mini((int)dp4a_u8(d0, d0, 0u), (int)dp4a_u8(d1, d1, 0u));
+        }
+    }
+    return total;
 }
 
 // Least-squares endpoints of one subset from its indices; K:1198-1262.  The sums are exact integers.
@@ -1071,29 +1172,33 @@ ITW_HD_NOINLINE void bc7_eval_shape(Bc7Warp& W, int lane, int slot, const Bc7Blo
                                             ends_b[3], ends_b[4], ends_b[5], chmask).err;
 }
 // ---- three-subset shapes (modes 0 and 2) -------------------------------------------------------------------
-// The 64 shapes x 3 subsets use only 140 distinct texel masks, and the PCA fit and the endpoint quantisation of a subset
-// depend on its mask alone (the reference refits per shape and per mode with identical results, K:1279-1297).  So, two
-// blocks at a time (`duo` = 0..3: blocks 2*duo, 2*duo+1 of the batch): phase A fits and quantises every distinct mask once
-// (lane <-> (block, mask)); phase B runs the index search of every shape from the stored endpoints (lane <-> (block, shape)).
-// Same values as evaluating shape by shape, 25 % fewer fits and quantisations.
+// The 64 shapes x 3 subsets use only 140 distinct texel masks, and the PCA fit, the endpoint quantisation and the index-search
+// error of a subset depend on its mask alone (the reference refits per shape and per mode with identical results,
+// K:1279-1297).  So, two blocks at a time (`duo` = 0..3: blocks 2*duo, 2*duo+1 of the batch): phase A fits and quantises
+// every distinct mask once and searches it for mode 2 (lane <-> (block, mask)); phase B adds up the mode-2 errors of every
+// shape's three masks and runs the mode-0 search of shapes 0..15 from the stored endpoints (lane <-> (block, shape)).  Same
+// values as evaluating shape by shape: 25 % fewer fits and quantisations, 27 % fewer mode-2 texels searched.  Mode 0 stays
+// per shape: its 72 masks of two blocks take three passes of short, divergent subset loops where its 32 shapes take one
+// dense pass, and that measured slower on the profiles that skip mode 2 (basic).
 ITW_HD void bc7_phase_masks3(int lane, Bc7Warp& W, const Bc7Params& P, int duo)
 {
     const int ca = bc7_slot_count(P, 0), cb = bc7_slot_count(P, 1);
     const int nmask = (cb > 0) ? ITW_MASK3_COUNT : ITW_MASK3_FIRST;
     const int nslots = mini(maxi(W.nvalid - 2 * duo, 0), 2);
     for (int t = lane; t < nslots * nmask; t += 32) {
-        const int s = t / nmask, u = t - s * nmask;
+        // the two blocks alternate, so that a step holds 16 masks of similar popcount
+        const int s = (nslots == 2) ? (t & 1) : 0, u = (nslots == 2) ? (t >> 1) : t;
         const Bc7Block* blk = &W.blk[2 * duo + s];
-        const Bc7Seg seg = bc7_fit(blk, 3, 1, (u32)ITW_TABLE(mask3_unique)[u], 3);
+        const u32 mask = ITW_TABLE(mask3_unique)[u];
+        const Bc7Seg seg = bc7_fit(blk, 3, 1, mask, 3);
         if (cb > 0) {
             const Bc7Packed pk = bc7_quantise(seg, 2, 3);
-            W.ends3.mode2[s][u][0] = pk.dec_a;
-            W.ends3.mode2[s][u][1] = pk.dec_b;
+            W.masks3.err2[s][u] = bc7_subset_error(blk, mask, pk.dec_a, pk.dec_b, 2);
         }
         if (ca > 0 && u < ITW_MASK3_FIRST) {
             const Bc7Packed pk = bc7_quantise(seg, 0, 3);
-            W.ends3.mode0[s][u][0] = pk.dec_a;
-            W.ends3.mode0[s][u][1] = pk.dec_b;
+            W.masks3.ends0[s][u][0] = pk.dec_a;
+            W.masks3.ends0[s][u][1] = pk.dec_b;
         }
     }
 }
@@ -1105,17 +1210,12 @@ ITW_HD void bc7_phase_shapes3(int lane, Bc7Warp& W, const Bc7Params& P, int duo)
     for (int t = lane; t < nslots * count; t += 32) {
         const int s = t / count, n = t - s * count;
         const int slot = (2 * duo + s) & (kBc7Slots - 1);             // scratch index inside the group
-        const Bc7Block* blk = &W.blk[2 * duo + s];
-        const u32 pattern = shape_pattern(64 + n);
         const int u0 = ITW_TABLE(shape3_mask_id)[3 * n], u1 = ITW_TABLE(shape3_mask_id)[3 * n + 1], u2 = ITW_TABLE(shape3_mask_id)[3 * n + 2];
+        const u32 (&e)[ITW_MASK3_FIRST][2] = W.masks3.ends0[s];
         if (n < ca)
-            W.cand_err[slot][0][n] = bc7_assign(W.palette, lane, blk, 3, 1, 3, 3, pattern, W.ends3.mode0[s][u0][0], W.ends3.mode0[s][u0][1],
-                                                W.ends3.mode0[s][u1][0], W.ends3.mode0[s][u1][1], W.ends3.mode0[s][u2][0],
-                                                W.ends3.mode0[s][u2][1], 0x00FFFFFFu).err;
-        if (n < cb)
-            W.cand_err[slot][1][n] = bc7_assign(W.palette, lane, blk, 3, 1, 2 | kAssignThresholds, 3, pattern, W.ends3.mode2[s][u0][0], W.ends3.mode2[s][u0][1],
-                                                W.ends3.mode2[s][u1][0], W.ends3.mode2[s][u1][1], W.ends3.mode2[s][u2][0],
-                                                W.ends3.mode2[s][u2][1], 0x00FFFFFFu).err;
+            W.cand_err[slot][0][n] = bc7_assign(W.palette, lane, &W.blk[2 * duo + s], 3, 1, 3, 3, shape_pattern(64 + n), e[u0][0], e[u0][1],
+                                                e[u1][0], e[u1][1], e[u2][0], e[u2][1], 0x00FFFFFFu).err;
+        if (n < cb) W.cand_err[slot][1][n] = W.masks3.err2[s][u0] + W.masks3.err2[s][u1] + W.masks3.err2[s][u2];
     }
 }
 
@@ -1146,18 +1246,55 @@ ITW_HD void bc7_phase_keys(int lane, Bc7Warp& W, const Bc7Params& P, int g, int 
     const int channels = (set == 0) ? 3 : P.channels;
     for (int t = lane; t < bc7_group_count(W, g) * 64; t += 32) {
         const int slot = t >> 6, shape = t & 63;
-        W.keys[slot][shape] = bc7_split_key(&W.blk[kBc7Slots * g + slot], shape, channels);
+        W.two.keys[slot][shape] = bc7_split_key(&W.blk[kBc7Slots * g + slot], shape, channels);
+    }
+}
+// ---- full two-subset lists (modes 1 and 3) ----------------------------------------------------------------------------
+// When the longer list holds all 64 shapes (max(t1, t3) = 64: the slow profiles), every shape is fitted and searched anyway
+// and the ranking only decides ties (the winner is the first minimum in ranked order).  Then, block by block: phase A fits
+// each of the 128 subset masks once (lane <-> mask), keeps the split bound its first four power iterations give, and
+// quantises and searches it for modes 1 and 3; phase B adds up the errors of every shape's two masks and forms its key from
+// the two bounds (lane <-> shape).  Shorter lists (basic: 12 and 8 shapes) rank first and then evaluate only the top t
+// shapes (bc7_phase_keys, bc7_phase_shapes), far fewer fits than the 128 masks.
+ITW_HD bool bc7_full_two(const Bc7Params& P) { return P.sel[1] && maxi(P.t1, P.t3) == 64; }
+ITW_HD void bc7_phase_masks2(int lane, Bc7Warp& W, const Bc7Params& P, int g, int slot)
+{
+    if (slot >= bc7_group_count(W, g)) return;
+    const Bc7Block* blk = &W.blk[kBc7Slots * g + slot];
+    for (int u = lane; u < 128; u += 32) {
+        const int id = ITW_TABLE(mask2_order)[u];
+        const u32 mask = (u32)shape_mask(id & 63, id >> 6);
+        const Bc7FitBound f = bc7_fit_bound(blk, mask);
+        W.two.bound[id] = f.bound;
+        if (P.t1 > 0) {
+            const Bc7Packed pk = bc7_quantise(f.seg, 1, 3);
+            W.two.mode1[id] = bc7_subset_error(blk, mask, pk.dec_a, pk.dec_b, 3);
+        }
+        if (P.t3 > 0) {
+            const Bc7Packed pk = bc7_quantise(f.seg, 3, 3);
+            W.two.mode3[id] = bc7_subset_error(blk, mask, pk.dec_a, pk.dec_b, 2);
+        }
+    }
+}
+ITW_HD void bc7_phase_shapes2(int lane, Bc7Warp& W, const Bc7Params& P, int g, int slot)
+{
+    if (slot >= bc7_group_count(W, g)) return;
+    for (int shape = lane; shape < 64; shape += 32) {
+        if (P.t1 > 0) W.cand_err[slot][0][shape] = W.two.mode1[shape] + W.two.mode1[64 + shape];
+        if (P.t3 > 0) W.cand_err[slot][1][shape] = W.two.mode3[shape] + W.two.mode3[64 + shape];
+        W.two.keys[slot][shape] = bc7_key_of(shape, W.two.bound[shape], W.two.bound[64 + shape]);
     }
 }
 ITW_HD void bc7_phase_rank(int lane, Bc7Warp& W, int g, int set)
 {
     for (int t = lane; t < bc7_group_count(W, g) * 64; t += 32) {
         const int slot = t >> 6, i = t & 63;
-        W.order[slot][set][rank_of(W.keys[slot], 64, i)] = (uint8_t)(W.keys[slot][i] & 63);
+        W.order[slot][set][rank_of(W.two.keys[slot], 64, i)] = (uint8_t)(W.two.keys[slot][i] & 63);
     }
 }
-// first minimum of the candidate lists just evaluated for mode slots (ma, mb) of group g, as a SHAPE id; K:1320 (strict <)
-ITW_HD void bc7_phase_winners(int lane, Bc7Warp& W, const Bc7Params& P, int g, int ma, int mb)
+// first minimum of the candidate lists just evaluated for mode slots (ma, mb) of group g, as a SHAPE id; K:1320 (strict <).
+// by_shape: the errors are stored by shape id, not by list position (bc7_phase_shapes2).
+ITW_HD void bc7_phase_winners(int lane, Bc7Warp& W, const Bc7Params& P, int g, int ma, int mb, bool by_shape)
 {
     const int nm = (mb != ma) ? 2 : 1;
     for (int t = lane; t < bc7_group_count(W, g) * nm; t += 32) {
@@ -1166,7 +1303,7 @@ ITW_HD void bc7_phase_winners(int lane, Bc7Warp& W, const Bc7Params& P, int g, i
         const int count = bc7_slot_count(P, m);
         int best = -1, best_err = kErrNone;
         for (int n = 0; n < count; n++) {
-            const int e = W.cand_err[slot][which][n];
+            const int e = W.cand_err[slot][which][by_shape ? bc7_slot_shape(W, slot, m, n) : n];
             if (e < best_err) { best_err = e; best = n; }
         }
         W.win_shape[kBc7Batch * W.half + kBc7Slots * g + slot][m] = (best < 0) ? -1 : bc7_slot_shape(W, slot, m, best);
@@ -1226,19 +1363,27 @@ ITW_HD void bc7_phase_store(int lane, Bc7Warp& W, const Bc7Params& P, uint8_t* d
         PHASE(bc7_phase_shapes3(lane, W, P, 2 * (g)));                                 \
         PHASE(bc7_phase_masks3(lane, W, P, 2 * (g) + 1));                              \
         PHASE(bc7_phase_shapes3(lane, W, P, 2 * (g) + 1));                             \
-        PHASE(bc7_phase_winners(lane, W, P, g, 0, 1));                                 \
+        PHASE(bc7_phase_winners(lane, W, P, g, 0, 1, false));                          \
     }                                                                                  \
-    if (bc7_needs_keys(P, 0)) {                                                        \
+    if (bc7_full_two(P)) {                                                             \
+        ITW_UNROLL(1)                                                                  \
+        for (int s = 0; s < kBc7Slots; s++) {                                          \
+            PHASE(bc7_phase_masks2(lane, W, P, g, s));                                 \
+            PHASE(bc7_phase_shapes2(lane, W, P, g, s));                                \
+        }                                                                              \
+        PHASE(bc7_phase_rank(lane, W, g, 0));                                          \
+        PHASE(bc7_phase_winners(lane, W, P, g, 2, 3, true));                           \
+    } else if (bc7_needs_keys(P, 0)) {                                                 \
         PHASE(bc7_phase_keys(lane, W, P, g, 0));                                       \
         PHASE(bc7_phase_rank(lane, W, g, 0));                                          \
         PHASE(bc7_phase_shapes(lane, W, P, g, 2, 3));                                  \
-        PHASE(bc7_phase_winners(lane, W, P, g, 2, 3));                                 \
+        PHASE(bc7_phase_winners(lane, W, P, g, 2, 3, false));                          \
     }                                                                                  \
     if (bc7_needs_keys(P, 1)) {                                                        \
         PHASE(bc7_phase_keys(lane, W, P, g, 1));                                       \
         PHASE(bc7_phase_rank(lane, W, g, 1));                                          \
         PHASE(bc7_phase_shapes(lane, W, P, g, 4, 4));                                  \
-        PHASE(bc7_phase_winners(lane, W, P, g, 4, 4));                                 \
+        PHASE(bc7_phase_winners(lane, W, P, g, 4, 4, false));                          \
     }
 // The halves and the groups are LOOPS, not copies: four inlined copies of every shape phase made the kernel body 6.6 k
 // instructions (105 KB) -- the phases of one copy are what the instruction cache should hold.
