@@ -8,10 +8,13 @@
 //   * shape phases: a shape's error is the sum of its subsets' errors, and a subset's fit, endpoints and error depend on its
 //     texel mask alone (the reference refits per shape and mode, K:1279-1297, with identical results).  So the three-subset
 //     shapes go lane <-> (block, distinct mask): fit once, quantise for modes 0 and 2 and search for mode 2, then lane <->
-//     (block, shape) adds three stored mode-2 errors and searches mode 0 from the stored endpoints.  The two-subset shapes
-//     (modes 1, 3) go lane <-> mask per block when the profile searches all 64 of them (the split keys then come from the
-//     fits' power iterations); for shorter lists and for mode 7 a lane evaluates one ranked shape: it fits each subset once
-//     and searches it for both modes of the pair;
+//     (block, shape) adds three stored mode-2 errors and searches mode 0 from the stored endpoints.  A two-subset shape
+//     (modes 1, 3, 7) belongs to one lane.  When the profile searches all 64 of them for modes 1 / 3, lane <-> (block, shape)
+//     over the four blocks of a group: one routine fits both subsets (bc7_fit_pair: subset 1's moments are the block's minus
+//     subset 0's, two independent power iterations, one projection loop) and gives the split keys, and one walk over the 16
+//     texels scores modes 1 and 3.  For shorter lists and for mode 7 a lane evaluates one ranked shape: it fits each subset
+//     and searches the shape for both modes of the pair (the pair fit measured slower there: it raises the register
+//     pressure of bc7_eval_shape);
 //   * ranking phase: lane <-> (block slot, two-subset shape) for the 64 PCA split bounds;
 //   * chain phase: lane <-> (block slot, role).  The per-mode refinement chains, the mode 4/5
 //     rotation / index-swap candidates and mode 6 are independent of one another in the reference
@@ -40,7 +43,6 @@
 // functions lane by lane on the CPU (test-only).
 #pragma once
 #include "bc67_core.cuh"
-#include "itw_masks2.cuh"
 #include "itw_masks3.cuh"
 
 // unroll factors of the two hottest loops; on H100 (tools/tune_unroll.sh) BC7 slow / basic take 33.65 / 13.51 ms at
@@ -57,8 +59,6 @@ namespace itw {
 // distinct subset masks of the three-subset shapes and the mask ids of each shape (tools/gen_mask_tables.py)
 ITW_TABLE_DECL(uint16_t, mask3_unique, ITW_MASK3_COUNT)
 ITW_TABLE_DECL(uint8_t, shape3_mask_id, 64 * 3)
-// the 128 subset masks of the two-subset shapes as shape + 64 * subset, ascending popcount (tools/gen_mask_tables.py)
-ITW_TABLE_DECL(uint8_t, mask2_order, 128)
 
 // bc7_enc_settings (ispc_texcomp.h:27-41) flattened to ints for the device
 struct Bc7Params {
@@ -108,10 +108,6 @@ struct Bc7Warp {
         // two-subset shapes of the group, after its three-subset phases
         struct {
             int keys[kBc7Slots][64];           // split-bound keys of the set being ranked: dead once `order` is written
-            // full lists (bc7_full_two), one block at a time: mode 1 / mode 3 errors and split bounds of the 128 subset
-            // masks, [shape + 64 * subset] (bc7_phase_masks2 -> bc7_phase_shapes2)
-            int mode1[128], mode3[128];
-            float bound[128];
         } two;
         // chain phase of a two-half round: the FIRST half again (re-read from the staged tile once its slot in blk[] has
         // been taken by the second half; the mask tables are dead by then)
@@ -356,14 +352,72 @@ ITW_HD_NOINLINE Bc7Seg bc7_fit(const Bc7Block* blk, int rot, int alpha, u32 mask
     else bc7_fit_impl<3, false>(seg.v, unused, v, mask);
     return seg;
 }
-// The three-channel fit of a subset of an untransformed block, and the split bound of its mask
-struct Bc7FitBound { Bc7Seg seg; float bound; };
-ITW_HD_NOINLINE Bc7FitBound bc7_fit_bound(const Bc7Block* blk, u32 mask)
+// Both subsets of a two-subset shape of an untransformed block: the same values as bc7_fit of mask0 and of its complement
+// (and, at three channels, their split bounds), with the work the two fits share done once.  Subset 1's integer moments are
+// the block's minus subset 0's (exact); the two covariance / power-iteration chains are independent, so the scheduler can
+// interleave them; one projection loop sends every texel to its own subset's axis and mean.
+struct Bc7Pair { Bc7Seg seg[2]; float bound[2]; };
+template <int CH, bool kBound>
+ITW_HD void bc7_fit_pair_impl(Bc7Pair& f, const Bc7Block* blk, u32 mask0)
 {
-    Bc7FitBound f;
+    static_assert(!kBound || CH == 3, "the four-channel fit adds eps to slot 9, the split bound does not");
+    u32 P[4][4];
+    load_planes(P, View{blk, 3, 1});
+    int full[15], part[15], rest[15];
+    moments_u8(full, P, 0xFFFFu, CH);
+    moments_u8(part, P, mask0, CH);
 #pragma unroll
-    for (int i = 0; i < 8; i++) f.seg.v[i] = 0.0f;
-    bc7_fit_impl<3, true>(f.seg.v, f.bound, View{blk, 3, 1}, mask);
+    for (int i = 0; i < 15; i++) rest[i] = full[i] - part[i];
+    float cov0[10], cov1[10], mean0[4], mean1[4];
+    bc7_covariance<CH>(cov0, mean0, part);
+    bc7_covariance<CH>(cov1, mean1, rest);
+    const float inv_var = 1.0f / (256.0f * 256.0f);
+#pragma unroll
+    for (int i = 0; i < 10; i++) { cov0[i] *= inv_var; cov1[i] *= inv_var; }
+    const float eps = 0.001f * 0.001f;
+    cov0[0] += eps; cov0[4] += eps; cov0[7] += eps; cov0[9] += eps;
+    cov1[0] += eps; cov1[4] += eps; cov1[7] += eps; cov1[9] += eps;
+    float axis0[4] = {1.0f, 1.0f, 1.0f, 1.0f}, axis1[4] = {1.0f, 1.0f, 1.0f, 1.0f};
+    bc7_power_axis<CH, 4>(axis0, cov0);
+    bc7_power_axis<CH, 4>(axis1, cov1);
+    f.bound[0] = f.bound[1] = 0.0f;
+    if (kBound) {
+        f.bound[0] = bc7_bound_from_axis<CH>(cov0, axis0);
+        f.bound[1] = bc7_bound_from_axis<CH>(cov1, axis1);
+    }
+    bc7_power_axis<CH, 4>(axis0, cov0);
+    bc7_power_axis<CH, 4>(axis1, cov1);
+
+    float lo0 = inf_f(), hi0 = -inf_f(), lo1 = inf_f(), hi1 = -inf_f();
+#pragma unroll
+    for (int k = 0; k < 16; k++) {
+        // bc7_fit_impl's projection with the texel's own subset's axis and mean: same operands, same order
+        const bool in0 = (mask0 >> k) & 1u;
+        float d = (in0 ? axis0[0] : axis1[0]) * ((float)((P[0][k >> 2] >> (8 * (k & 3))) & 255u) - (in0 ? mean0[0] : mean1[0]));
+#pragma unroll
+        for (int c = 1; c < CH; c++)
+            d += (in0 ? axis0[c] : axis1[c]) * ((float)((P[c][k >> 2] >> (8 * (k & 3))) & 255u) - (in0 ? mean0[c] : mean1[c]));
+        if (in0) { lo0 = fminf(lo0, d); hi0 = fmaxf(hi0, d); }
+        else     { lo1 = fminf(lo1, d); hi1 = fmaxf(hi1, d); }
+    }
+    if (hi0 - lo0 < 1.0f) { lo0 -= 0.5f; hi0 += 0.5f; }
+    if (hi1 - lo1 < 1.0f) { lo1 -= 0.5f; hi1 += 0.5f; }
+#pragma unroll
+    for (int i = 0; i < 8; i++) f.seg[0].v[i] = f.seg[1].v[i] = 0.0f;
+#pragma unroll
+    for (int c = 0; c < CH; c++) {
+        f.seg[0].v[c] = clamp_sse(lo0 * axis0[c] + mean0[c], 0.0f, 255.0f);
+        f.seg[0].v[4 + c] = clamp_sse(hi0 * axis0[c] + mean0[c], 0.0f, 255.0f);
+        f.seg[1].v[c] = clamp_sse(lo1 * axis1[c] + mean1[c], 0.0f, 255.0f);
+        f.seg[1].v[4 + c] = clamp_sse(hi1 * axis1[c] + mean1[c], 0.0f, 255.0f);
+    }
+}
+// mask0 = subset 0 of a two-subset shape; bound[] is set at three channels only
+ITW_HD_NOINLINE Bc7Pair bc7_fit_pair(const Bc7Block* blk, u32 mask0, int channels)
+{
+    Bc7Pair f;
+    if (channels == 4) bc7_fit_pair_impl<4, false>(f, blk, mask0);
+    else bc7_fit_pair_impl<3, true>(f, blk, mask0);
     return f;
 }
 
@@ -632,54 +686,88 @@ ITW_HD_NOINLINE Bc7Search bc7_assign(u32 (*pal)[32], int lane, const Bc7Block* b
     }
     return Bc7Search{total, out0, out1};
 }
-// Error of ONE subset of a shape-phase search (three channels, untransformed block): bc7_assign's arithmetic -- the
-// integer-threshold two-bit form, the FMA-corrected quotient for three bits, VABSDIFF4 + IDP.4A errors -- over the texels of
-// `mask` only, with the subset's constants and palette in registers and no index bits.  The error of a shape is the sum of
-// the errors of its subsets (exact integers), and a subset's endpoints depend on its mask alone, so the shape phases search
-// every distinct mask once (modes 1, 2, 3).  The first-of-two choice adds min(e0, e1).
-ITW_HD_NOINLINE int bc7_subset_error(const Bc7Block* blk, u32 mask, u32 dec_a, u32 dec_b, int bits)
+// Shape-phase searches without index bits (three channels, untransformed block): bc7_assign's arithmetic -- the
+// integer-threshold two-bit form, the FMA-corrected quotient for three bits, VABSDIFF4 + IDP.4A errors -- with each subset's
+// constants and palette in registers.  The error of a shape is the sum of the errors of its subsets (exact integers); the
+// first-of-two choice adds min(e0, e1).
+// Two-bit constants of one subset: q1 = 1 + (num >= t2) + (num >= t3), t2 <= t3 (thresholds as in bc7_assign)
+struct Bc7Sub2 { u32 a, b; int cj, t2, t3; u32 p1, p2; };
+ITW_HD Bc7Sub2 bc7_sub2(u32 dec_a, u32 dec_b)
 {
     const u32 a = dec_a & 0x00FFFFFFu, b = dec_b & 0x00FFFFFFu;
     const u32 aa = dp4a_u8(a, a, 0u), ab = dp4a_u8(a, b, 0u), bb = dp4a_u8(b, b, 0u);
-    const int idiv = (int)(bb - 2u * ab + aa), cj = (int)(ab - aa);
+    const int idiv = (int)(bb - 2u * ab + aa);
     const Bc7Lerp lerp = bc7_lerp(a, b);
-    // a counted loop over the set bits, unrolled so that the texel loads of several iterations are in flight at once (a
-    // rolled loop waits for each load: four warps per scheduler do not hide that latency)
+    return Bc7Sub2{a, b, (int)(ab - aa), idiv ? (3 * idiv + 7) >> 3 : 0x7fffffff, idiv ? (5 * idiv + 7) >> 3 : 0x7fffffff,
+                   lerp.entry((u32)bc7_weight(2, 1)), lerp.entry((u32)bc7_weight(2, 2))};
+}
+ITW_HD int bc7_texel_error2(const Bc7Sub2& s, u32 t)
+{
+    const int num = (int)dp4a_u8(t, s.b, 0u) - (int)dp4a_u8(t, s.a, 0u) - s.cj;
+    const bool ge2 = num >= s.t2, ge3 = num >= s.t3;
+    const u32 lo = ge3 ? s.p2 : (ge2 ? s.p1 : s.a), hi = ge3 ? s.b : (ge2 ? s.p2 : s.p1);      // palette entries q1 - 1, q1
+    const u32 d0 = absdiff_u8x4(lo, t), d1 = absdiff_u8x4(hi, t);
+    return mini((int)dp4a_u8(d0, d0, 0u), (int)dp4a_u8(d1, d1, 0u));
+}
+// Three-bit constants of one subset
+struct Bc7Sub3 { u32 a, b; int cj; float fdiv, rdiv; Bc7Lerp lerp; };
+ITW_HD Bc7Sub3 bc7_sub3(u32 dec_a, u32 dec_b)
+{
+    const u32 a = dec_a & 0x00FFFFFFu, b = dec_b & 0x00FFFFFFu;
+    const u32 aa = dp4a_u8(a, a, 0u), ab = dp4a_u8(a, b, 0u), bb = dp4a_u8(b, b, 0u);
+    const float fdiv = (float)(int)(bb - 2u * ab + aa);
+    return Bc7Sub3{a, b, (int)(ab - aa), fdiv, 1.0f / fdiv, bc7_lerp(a, b)};
+}
+ITW_HD int bc7_texel_error3(const Bc7Sub3& s, u32 t)
+{
+    const int num = (int)dp4a_u8(t, s.b, 0u) - (int)dp4a_u8(t, s.a, 0u) - s.cj;
+    const float proj = div_by_rcp((float)num, s.fdiv, s.rdiv);
+    const int q1 = clampi(trunc_i(fma_rn(proj, 8.0f, 0.5f)), 1, 7);
+    const u32 lo = s.lerp.entry((u32)bc7_weight(3, q1 - 1)), hi = s.lerp.entry((u32)bc7_weight(3, q1));
+    const u32 d0 = absdiff_u8x4(lo, t), d1 = absdiff_u8x4(hi, t);
+    return mini((int)dp4a_u8(d0, d0, 0u), (int)dp4a_u8(d1, d1, 0u));
+}
+// Mode-2 error of ONE subset mask: a subset's endpoints depend on its mask alone, so the three-subset phases search every
+// distinct mask once.  A counted loop over the set bits, unrolled so that the texel loads of several iterations are in
+// flight at once (a rolled loop waits for each load: four warps per scheduler do not hide that latency).
+ITW_HD_NOINLINE int bc7_subset_error(const Bc7Block* blk, u32 mask, u32 dec_a, u32 dec_b)
+{
+    const Bc7Sub2 s = bc7_sub2(dec_a, dec_b);
     const int n = popcount16(mask);
     int total = 0;
-    if (bits == 2) {
-        // thresholds as in bc7_assign: q1 = 1 + (num >= t2) + (num >= t3), t2 <= t3
-        const int t2 = idiv ? (3 * idiv + 7) >> 3 : 0x7fffffff, t3 = idiv ? (5 * idiv + 7) >> 3 : 0x7fffffff;
-        const u32 p1 = lerp.entry((u32)bc7_weight(2, 1)), p2 = lerp.entry((u32)bc7_weight(2, 2));
-        u32 rest = mask;
+    u32 rest = mask;
 #pragma unroll 4
-        for (int i = 0; i < n; i++) {
-            const u32 low = rest & (0u - rest);
-            rest ^= low;
-            const u32 t = blk->rgb[popcount32(low - 1u)];
-            const int num = (int)dp4a_u8(t, b, 0u) - (int)dp4a_u8(t, a, 0u) - cj;
-            const bool ge2 = num >= t2, ge3 = num >= t3;
-            const u32 lo = ge3 ? p2 : (ge2 ? p1 : a), hi = ge3 ? b : (ge2 ? p2 : p1);      // palette entries q1 - 1, q1
-            const u32 d0 = absdiff_u8x4(lo, t), d1 = absdiff_u8x4(hi, t);
-            total += mini((int)dp4a_u8(d0, d0, 0u), (int)dp4a_u8(d1, d1, 0u));
-        }
-    } else {
-        const float fdiv = (float)idiv, rdiv = 1.0f / fdiv;
-        u32 rest = mask;
-#pragma unroll 4
-        for (int i = 0; i < n; i++) {
-            const u32 low = rest & (0u - rest);
-            rest ^= low;
-            const u32 t = blk->rgb[popcount32(low - 1u)];
-            const int num = (int)dp4a_u8(t, b, 0u) - (int)dp4a_u8(t, a, 0u) - cj;
-            const float proj = div_by_rcp((float)num, fdiv, rdiv);
-            const int q1 = clampi(trunc_i(fma_rn(proj, 8.0f, 0.5f)), 1, 7);
-            const u32 lo = lerp.entry((u32)bc7_weight(3, q1 - 1)), hi = lerp.entry((u32)bc7_weight(3, q1));
-            const u32 d0 = absdiff_u8x4(lo, t), d1 = absdiff_u8x4(hi, t);
-            total += mini((int)dp4a_u8(d0, d0, 0u), (int)dp4a_u8(d1, d1, 0u));
-        }
+    for (int i = 0; i < n; i++) {
+        const u32 low = rest & (0u - rest);
+        rest ^= low;
+        total += bc7_texel_error2(s, blk->rgb[popcount32(low - 1u)]);
     }
     return total;
+}
+// Mode-1 (three-bit) and mode-3 (two-bit) errors of one two-subset shape, mask0 = its subset 0: one walk over the 16 texels,
+// each scored against its own subset's constants.  e1 / e3 = decoded endpoints A, B of subsets 0 and 1 for mode 1 / mode 3.
+struct Bc7PairErr { int mode1, mode3; };
+ITW_HD_NOINLINE Bc7PairErr bc7_pair_error(const Bc7Block* blk, u32 mask0, u32 e1a0, u32 e1b0, u32 e1a1, u32 e1b1, u32 e3a0,
+                                          u32 e3b0, u32 e3a1, u32 e3b1)
+{
+    const Bc7Sub3 m1s0 = bc7_sub3(e1a0, e1b0), m1s1 = bc7_sub3(e1a1, e1b1);
+    const Bc7Sub2 m3s0 = bc7_sub2(e3a0, e3b0), m3s1 = bc7_sub2(e3a1, e3b1);
+    int total1 = 0, total3 = 0;
+    ITW_UNROLL(ITW_BC7_ASSIGN_UNROLL)
+    for (int k = 0; k < 16; k++) {
+        const u32 t = blk->rgb[k];
+        const bool in0 = (mask0 >> k) & 1u;
+        // field by field: a select of whole structs would take their addresses and put both in local memory
+        const Bc7Sub3 s1{in0 ? m1s0.a : m1s1.a, in0 ? m1s0.b : m1s1.b, in0 ? m1s0.cj : m1s1.cj, in0 ? m1s0.fdiv : m1s1.fdiv,
+                         in0 ? m1s0.rdiv : m1s1.rdiv,
+                         Bc7Lerp{in0 ? m1s0.lerp.base_rb : m1s1.lerp.base_rb, in0 ? m1s0.lerp.base_ga : m1s1.lerp.base_ga,
+                                 in0 ? m1s0.lerp.d_rb : m1s1.lerp.d_rb, in0 ? m1s0.lerp.d_ga : m1s1.lerp.d_ga}};
+        const Bc7Sub2 s3{in0 ? m3s0.a : m3s1.a, in0 ? m3s0.b : m3s1.b, in0 ? m3s0.cj : m3s1.cj, in0 ? m3s0.t2 : m3s1.t2,
+                         in0 ? m3s0.t3 : m3s1.t3, in0 ? m3s0.p1 : m3s1.p1, in0 ? m3s0.p2 : m3s1.p2};
+        total1 += bc7_texel_error3(s1, t);
+        total3 += bc7_texel_error2(s3, t);
+    }
+    return Bc7PairErr{total1, total3};
 }
 
 // Least-squares endpoints of one subset from its indices; K:1198-1262.  The sums are exact integers.
@@ -1139,20 +1227,19 @@ ITW_HD void bc7_phase_planes(int lane, Bc7Warp& W)
         W.blk[slot].plane[c][i] = v;
     }
 }
-// One shape, both modes of a mode-slot pair (ma, mb): fits once, quantises and searches per mode.  `slot` = position inside
-// the group (scratch index), `blk` = the block.
+// One two-subset shape, both modes of a mode-slot pair (ma, mb) -- modes 1 and 3, or mode 7: fits once, quantises and searches
+// per mode.  `slot` = position inside the group (scratch index), `blk` = the block.
 ITW_HD_NOINLINE void bc7_eval_shape(Bc7Warp& W, int lane, int slot, const Bc7Block* blk, int shape, int n, int ma, bool do_a, int mb, bool do_b)
 {
     const int mode_a = bc7_slot_mode(ma), mode_b = bc7_slot_mode(mb);
-    const int pairs = bc7_pairs(mode_a);
+    const int pairs = 2;
     const int channels = (mode_a == 7) ? 4 : 3;
     const u32 chmask = (channels == 4) ? 0xFFFFFFFFu : 0x00FFFFFFu;
     u32 ends_a[6], ends_b[6];
 #pragma unroll
     for (int i = 0; i < 6; i++) ends_a[i] = ends_b[i] = 0u;
 #pragma unroll
-    for (int j = 0; j < 3; j++) {
-        if (j >= pairs) continue;
+    for (int j = 0; j < 2; j++) {
         const Bc7Seg seg = bc7_fit(blk, 3, 1, (u32)shape_mask(shape, j), channels);
         if (do_a) {
             const Bc7Packed pk = bc7_quantise(seg, mode_a, channels);
@@ -1193,7 +1280,7 @@ ITW_HD void bc7_phase_masks3(int lane, Bc7Warp& W, const Bc7Params& P, int duo)
         const Bc7Seg seg = bc7_fit(blk, 3, 1, mask, 3);
         if (cb > 0) {
             const Bc7Packed pk = bc7_quantise(seg, 2, 3);
-            W.masks3.err2[s][u] = bc7_subset_error(blk, mask, pk.dec_a, pk.dec_b, 2);
+            W.masks3.err2[s][u] = bc7_subset_error(blk, mask, pk.dec_a, pk.dec_b);
         }
         if (ca > 0 && u < ITW_MASK3_FIRST) {
             const Bc7Packed pk = bc7_quantise(seg, 0, 3);
@@ -1251,38 +1338,35 @@ ITW_HD void bc7_phase_keys(int lane, Bc7Warp& W, const Bc7Params& P, int g, int 
 }
 // ---- full two-subset lists (modes 1 and 3) ----------------------------------------------------------------------------
 // When the longer list holds all 64 shapes (max(t1, t3) = 64: the slow profiles), every shape is fitted and searched anyway
-// and the ranking only decides ties (the winner is the first minimum in ranked order).  Then, block by block: phase A fits
-// each of the 128 subset masks once (lane <-> mask), keeps the split bound its first four power iterations give, and
-// quantises and searches it for modes 1 and 3; phase B adds up the errors of every shape's two masks and forms its key from
-// the two bounds (lane <-> shape).  Shorter lists (basic: 12 and 8 shapes) rank first and then evaluate only the top t
-// shapes (bc7_phase_keys, bc7_phase_shapes), far fewer fits than the 128 masks.
+// and the ranking only decides ties (the winner is the first minimum in ranked order).  Then lane <-> (block, shape) over the
+// whole group: one pair fit (whose first four power iterations give both split bounds, hence the key), quantisation of both
+// subsets for modes 1 and 3, and one walk over the 16 texels for both modes' errors.  Shorter lists (basic: 12 and 8 shapes)
+// rank first and then evaluate only the top t shapes (bc7_phase_keys, bc7_phase_shapes), far fewer fits than all 64.
 ITW_HD bool bc7_full_two(const Bc7Params& P) { return P.sel[1] && maxi(P.t1, P.t3) == 64; }
-ITW_HD void bc7_phase_masks2(int lane, Bc7Warp& W, const Bc7Params& P, int g, int slot)
+ITW_HD void bc7_phase_two_full(int lane, Bc7Warp& W, const Bc7Params& P, int g)
 {
-    if (slot >= bc7_group_count(W, g)) return;
-    const Bc7Block* blk = &W.blk[kBc7Slots * g + slot];
-    for (int u = lane; u < 128; u += 32) {
-        const int id = ITW_TABLE(mask2_order)[u];
-        const u32 mask = (u32)shape_mask(id & 63, id >> 6);
-        const Bc7FitBound f = bc7_fit_bound(blk, mask);
-        W.two.bound[id] = f.bound;
-        if (P.t1 > 0) {
-            const Bc7Packed pk = bc7_quantise(f.seg, 1, 3);
-            W.two.mode1[id] = bc7_subset_error(blk, mask, pk.dec_a, pk.dec_b, 3);
+    for (int t = lane; t < bc7_group_count(W, g) * 64; t += 32) {
+        const int slot = t >> 6, shape = t & 63;
+        const Bc7Block* blk = &W.blk[kBc7Slots * g + slot];
+        const u32 mask0 = (u32)shape_mask(shape, 0);
+        const Bc7Pair f = bc7_fit_pair(blk, mask0, 3);
+        // a list the profile leaves empty walks zero endpoints and is not stored
+        u32 e1[4] = {0u, 0u, 0u, 0u}, e3[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+        for (int j = 0; j < 2; j++) {
+            if (P.t1 > 0) {
+                const Bc7Packed pk = bc7_quantise(f.seg[j], 1, 3);
+                e1[2 * j] = pk.dec_a; e1[2 * j + 1] = pk.dec_b;
+            }
+            if (P.t3 > 0) {
+                const Bc7Packed pk = bc7_quantise(f.seg[j], 3, 3);
+                e3[2 * j] = pk.dec_a; e3[2 * j + 1] = pk.dec_b;
+            }
         }
-        if (P.t3 > 0) {
-            const Bc7Packed pk = bc7_quantise(f.seg, 3, 3);
-            W.two.mode3[id] = bc7_subset_error(blk, mask, pk.dec_a, pk.dec_b, 2);
-        }
-    }
-}
-ITW_HD void bc7_phase_shapes2(int lane, Bc7Warp& W, const Bc7Params& P, int g, int slot)
-{
-    if (slot >= bc7_group_count(W, g)) return;
-    for (int shape = lane; shape < 64; shape += 32) {
-        if (P.t1 > 0) W.cand_err[slot][0][shape] = W.two.mode1[shape] + W.two.mode1[64 + shape];
-        if (P.t3 > 0) W.cand_err[slot][1][shape] = W.two.mode3[shape] + W.two.mode3[64 + shape];
-        W.two.keys[slot][shape] = bc7_key_of(shape, W.two.bound[shape], W.two.bound[64 + shape]);
+        const Bc7PairErr e = bc7_pair_error(blk, mask0, e1[0], e1[1], e1[2], e1[3], e3[0], e3[1], e3[2], e3[3]);
+        if (P.t1 > 0) W.cand_err[slot][0][shape] = e.mode1;
+        if (P.t3 > 0) W.cand_err[slot][1][shape] = e.mode3;
+        W.two.keys[slot][shape] = bc7_key_of(shape, f.bound[0], f.bound[1]);
     }
 }
 ITW_HD void bc7_phase_rank(int lane, Bc7Warp& W, int g, int set)
@@ -1293,7 +1377,7 @@ ITW_HD void bc7_phase_rank(int lane, Bc7Warp& W, int g, int set)
     }
 }
 // first minimum of the candidate lists just evaluated for mode slots (ma, mb) of group g, as a SHAPE id; K:1320 (strict <).
-// by_shape: the errors are stored by shape id, not by list position (bc7_phase_shapes2).
+// by_shape: the errors are stored by shape id, not by list position (bc7_phase_two_full).
 ITW_HD void bc7_phase_winners(int lane, Bc7Warp& W, const Bc7Params& P, int g, int ma, int mb, bool by_shape)
 {
     const int nm = (mb != ma) ? 2 : 1;
@@ -1366,11 +1450,7 @@ ITW_HD void bc7_phase_store(int lane, Bc7Warp& W, const Bc7Params& P, uint8_t* d
         PHASE(bc7_phase_winners(lane, W, P, g, 0, 1, false));                          \
     }                                                                                  \
     if (bc7_full_two(P)) {                                                             \
-        ITW_UNROLL(1)                                                                  \
-        for (int s = 0; s < kBc7Slots; s++) {                                          \
-            PHASE(bc7_phase_masks2(lane, W, P, g, s));                                 \
-            PHASE(bc7_phase_shapes2(lane, W, P, g, s));                                \
-        }                                                                              \
+        PHASE(bc7_phase_two_full(lane, W, P, g));                                      \
         PHASE(bc7_phase_rank(lane, W, g, 0));                                          \
         PHASE(bc7_phase_winners(lane, W, P, g, 2, 3, true));                           \
     } else if (bc7_needs_keys(P, 0)) {                                                 \
