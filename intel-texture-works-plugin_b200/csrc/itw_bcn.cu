@@ -14,6 +14,7 @@
 #include <cstdio>
 #include <cstring>
 #include <functional>
+#include <initializer_list>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -35,14 +36,21 @@ namespace {
 std::atomic<uint64_t> g_launches{0};
 std::atomic<int> g_default_device{-1};      // itw_set_devices() with ONE device: the process-wide default
 
-struct ThreadCtx {
+inline int pad4(int v) { return (v + 3) & ~3; }
+template <typename T> inline T lvl(T v, int l) { v >>= l; return v ? v : 1; }      // size of mip level l
+inline bool pow2_dims(int w, int h) { return (w & (w - 1)) == 0 && (h & (h - 1)) == 0; }   // GenerateMipMaps then box-filters
+
+// Device staging of one surface encode: host rows go to d_in, blocks that cannot go straight to dst come back through d_out.
+struct Staging {
+    uint8_t* d_in = nullptr;  size_t d_in_cap = 0;
+    uint8_t* d_out = nullptr; size_t d_out_cap = 0;
+};
+struct ThreadCtx : Staging {
     int device = -1;             // device the resources below belong to
     int wanted_device = -1;      // itw_set_device() request, -1 = keep the current device
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     bool timed = false;
-    uint8_t* d_in = nullptr;  size_t d_in_cap = 0;
-    uint8_t* d_out = nullptr; size_t d_out_cap = 0;
     uint8_t* d_mid = nullptr; size_t d_mid_cap = 0;      // itw_encode_pixels: the converted surface between the two kernels
     // band pipeline of the compute-bound encoders (encode_banded): copy-in / copy-out streams and per-band events
     cudaStream_t copy_in = nullptr, copy_out = nullptr;
@@ -51,10 +59,8 @@ struct ThreadCtx {
     std::string err;
     // itw_encode_batch: three copy/compute lanes so that H2D of tile i+1, the kernel of tile i and
     // D2H of tile i-1 overlap (tile streaming, SURVEY.md 8e)
-    struct Lane {
+    struct Lane : Staging {
         cudaStream_t stream = nullptr;
-        uint8_t* d_in = nullptr;  size_t d_in_cap = 0;
-        uint8_t* d_out = nullptr; size_t d_out_cap = 0;
         bool busy = false;
     } lanes[3];
     // deferred mode (itw_begin_deferred / itw_flush): host calls are enqueued on the lanes round-robin and drained by itw_flush
@@ -100,6 +106,20 @@ int fail(const char* what, cudaError_t e = cudaSuccess)
         if (e_ != cudaSuccess) return fail(#call, e_);             \
     } while (0)
 
+// A call that enqueued work on its own streams leaves through drain(), also after an error: the caller may free src / dst
+// as soon as it returns, and the staging buffers must be idle for the next call.  The first failing step is the one reported.
+struct FirstError {
+    int rc = 0;
+    bool step(cudaError_t e, const char* what) { if (rc == 0 && e != cudaSuccess) rc = fail(what, e); return rc == 0; }
+    bool step(int r) { if (rc == 0 && r) rc = -1; return rc == 0; }        // r from a helper that reported through fail()
+    int drain(std::initializer_list<cudaStream_t> streams)
+    {
+        for (cudaStream_t s : streams) step(cudaStreamSynchronize(s), "cudaStreamSynchronize");
+        if (rc) cudaGetLastError();
+        return rc;
+    }
+};
+
 int ensure_ctx()
 {
     ThreadCtx& c = tls;
@@ -126,6 +146,10 @@ int ensure_ctx()
     ITW_CUDA(cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking));
     ITW_CUDA(cudaEventCreate(&c.ev0));
     ITW_CUDA(cudaEventCreate(&c.ev1));
+    ITW_CUDA(cudaFuncSetAttribute(bc7_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBc7SmemBytes));
+    ITW_CUDA(cudaFuncSetAttribute(bc7_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBc7SmemBytes));
+    ITW_CUDA(cudaFuncSetAttribute(bc6h_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBc6SmemBytes));
+    ITW_CUDA(cudaFuncSetAttribute(bc6h_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBc6SmemBytes));
     c.device = dev;
     return 0;
 }
@@ -168,14 +192,36 @@ int check_surface(const rgba_surface* s, const FormatInfo& f)
     return 0;
 }
 
-// Enqueue the kernel for one device-resident surface on `stream`.
-int launch(int format, const SurfaceView& v, uint8_t* d_dst, const void* settings, cudaStream_t stream)
+// An encoder resolved from (format, settings) before anything is enqueued: launch() can then fail only on a CUDA error.
+struct Encoder {
+    int format;                  // BC6H_SF16 is encoded by the unsigned encoder (IntelPlugin.cpp:840-843)
+    FormatInfo f;
+    Bc7Params bc7;
+    Bc6Params bc6;
+};
+int resolve_encoder(int format, const void* settings, Encoder& e)
 {
-    if (format == ITW_FORMAT_BC6H_SF16) format = ITW_FORMAT_BC6H;     // the plug-in encodes SF16 with the unsigned encoder (IntelPlugin.cpp:840-843)
+    e.format = format == ITW_FORMAT_BC6H_SF16 ? ITW_FORMAT_BC6H : format;
+    if (!format_info(e.format, e.f)) return fail("unknown format");
+    if (e.format == ITW_FORMAT_BC7) {
+        if (!settings) return fail("CompressBlocksBC7: null settings");
+        e.bc7 = bc7_params_from(*static_cast<const bc7_enc_settings*>(settings));
+        if (const char* why = bc7_params_check(e.bc7)) return fail(why);
+    } else if (e.format == ITW_FORMAT_BC6H) {
+        if (!settings) return fail("CompressBlocksBC6H: null settings");
+        e.bc6 = bc6_params_from(*static_cast<const bc6h_enc_settings*>(settings));
+        if (const char* why = bc6_params_check(e.bc6)) return fail(why);
+    }
+    return 0;
+}
+
+// Enqueue the kernel for one device-resident surface on `stream`.
+int launch(const Encoder& e, const SurfaceView& v, uint8_t* d_dst, cudaStream_t stream)
+{
     const long long nblocks = (long long)(v.width >> 2) * (v.height >> 2);
     const bool vec16 = ((reinterpret_cast<uintptr_t>(v.ptr) | (uintptr_t)v.stride) & 15u) == 0;
     const unsigned grid1 = (unsigned)((nblocks + 127) / 128);
-    switch (format) {
+    switch (e.format) {
         case ITW_FORMAT_BC1:
             if (vec16) bc1_bc3_kernel<false, true><<<grid1, 128, 0, stream>>>(v, d_dst);
             else       bc1_bc3_kernel<false, false><<<grid1, 128, 0, stream>>>(v, d_dst);
@@ -193,9 +239,6 @@ int launch(int format, const SurfaceView& v, uint8_t* d_dst, const void* setting
             else       bc4_bc5_kernel<true, false><<<grid1, 128, 0, stream>>>(v, d_dst);
             break;
         case ITW_FORMAT_BC7: {
-            if (!settings) return fail("CompressBlocksBC7: null settings");
-            const Bc7Params P = bc7_params_from(*static_cast<const bc7_enc_settings*>(settings));
-            if (const char* why = bc7_params_check(P)) return fail(why);
             // one 16-warp CTA per SM, persistent over the rounds; TMA-staged variant when the surface allows it.  A warp takes 16
             // blocks per round when that still gives every SM a full CTA, else 8 (small surfaces / row bands: more warps busy)
             const bool tma = vec16;                                       // 16-byte aligned rows
@@ -204,33 +247,18 @@ int launch(int format, const SurfaceView& v, uint8_t* d_dst, const void* setting
             const long long tile = (long long)kBc7WarpsPerCta * per_warp;
             const long long want = (nblocks + tile - 1) / tile;
             const unsigned grid = (unsigned)(want < cap ? want : cap);
-            // per-device attribute; cheap enough to set on every (millisecond-scale) launch
-            if (tma) {
-                ITW_CUDA(cudaFuncSetAttribute(bc7_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBc7SmemBytes));
-                bc7_kernel<true><<<grid, kBc7WarpsPerCta * 32, kBc7SmemBytes, stream>>>(v, d_dst, P, nblocks, per_warp);
-            } else {
-                ITW_CUDA(cudaFuncSetAttribute(bc7_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBc7SmemBytes));
-                bc7_kernel<false><<<grid, kBc7WarpsPerCta * 32, kBc7SmemBytes, stream>>>(v, d_dst, P, nblocks, per_warp);
-            }
+            if (tma) bc7_kernel<true><<<grid, kBc7WarpsPerCta * 32, kBc7SmemBytes, stream>>>(v, d_dst, e.bc7, nblocks, per_warp);
+            else     bc7_kernel<false><<<grid, kBc7WarpsPerCta * 32, kBc7SmemBytes, stream>>>(v, d_dst, e.bc7, nblocks, per_warp);
             break;
         }
         case ITW_FORMAT_BC6H: {
-            if (!settings) return fail("CompressBlocksBC6H: null settings");
-            const Bc6Params P = bc6_params_from(*static_cast<const bc6h_enc_settings*>(settings));
-            if (const char* why = bc6_params_check(P)) return fail(why);
             const long long want = (nblocks + kBc6TileBlocks - 1) / kBc6TileBlocks;
             const long long cap = (long long)tls.sm_count;
             const unsigned grid = (unsigned)(want < cap ? want : cap);
-            if (vec16) {
-                ITW_CUDA(cudaFuncSetAttribute(bc6h_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBc6SmemBytes));
-                bc6h_kernel<true><<<grid, kBc6WarpsPerCta * 32, kBc6SmemBytes, stream>>>(v, d_dst, P, nblocks);
-            } else {
-                ITW_CUDA(cudaFuncSetAttribute(bc6h_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBc6SmemBytes));
-                bc6h_kernel<false><<<grid, kBc6WarpsPerCta * 32, kBc6SmemBytes, stream>>>(v, d_dst, P, nblocks);
-            }
+            if (vec16) bc6h_kernel<true><<<grid, kBc6WarpsPerCta * 32, kBc6SmemBytes, stream>>>(v, d_dst, e.bc6, nblocks);
+            else       bc6h_kernel<false><<<grid, kBc6WarpsPerCta * 32, kBc6SmemBytes, stream>>>(v, d_dst, e.bc6, nblocks);
             break;
         }
-        default: return fail("unknown format");
     }
     g_launches.fetch_add(1, std::memory_order_relaxed);
     ITW_CUDA(cudaGetLastError());
@@ -239,12 +267,43 @@ int launch(int format, const SurfaceView& v, uint8_t* d_dst, const void* setting
 
 int encode_many(int format, const rgba_surface* srcs, uint8_t* const* dsts, int count, const void* settings);
 
+// Host rows -> tight device rows: one linear copy when the rows are already tight (full PCIe rate from pinned memory), else 2-D.
+cudaError_t copy_rows_h2d(uint8_t* d, const void* h, size_t h_stride, size_t row_bytes, size_t rows, cudaStream_t s)
+{
+    if (h_stride == row_bytes) return cudaMemcpyAsync(d, h, row_bytes * rows, cudaMemcpyHostToDevice, s);
+    return cudaMemcpy2DAsync(d, row_bytes, h, h_stride, row_bytes, rows, cudaMemcpyHostToDevice, s);
+}
+
+// One surface encode on `s` through a staging pair: a host source is copied into d_in, then the launch, then the blocks go
+// straight into a 16-byte aligned device dst or through d_out and a copy back.  ev0 / ev1, when given, bracket the launch for
+// itw_last_kernel_ms.  Returns false after the first failing step; the caller drains `s`.
+bool encode_surface(FirstError& fe, const Encoder& e, const rgba_surface* src, bool src_dev, uint8_t* dst, bool dst_dev, Staging& b,
+                    cudaStream_t s, cudaEvent_t ev0 = nullptr, cudaEvent_t ev1 = nullptr)
+{
+    const size_t row_bytes = (size_t)src->width * e.f.texel_bytes;
+    const size_t out_bytes = (size_t)(src->width >> 2) * (src->height >> 2) * e.f.bpb;
+    const bool dst_direct = dst_dev && (reinterpret_cast<uintptr_t>(dst) & 15u) == 0;
+    if (!src_dev && !fe.step(grow(b.d_in, b.d_in_cap, row_bytes * src->height))) return false;
+    if (!dst_direct && !fe.step(grow(b.d_out, b.d_out_cap, out_bytes))) return false;
+    SurfaceView v{src->ptr, src->width, src->height, src->stride};
+    if (!src_dev) {
+        if (!fe.step(copy_rows_h2d(b.d_in, src->ptr, (size_t)src->stride, row_bytes, (size_t)src->height, s), "H2D")) return false;
+        v.ptr = b.d_in;
+        v.stride = (int)row_bytes;
+    }
+    uint8_t* d_dst = dst_direct ? dst : b.d_out;
+    if (ev0 && !fe.step(cudaEventRecord(ev0, s), "cudaEventRecord")) return false;
+    if (!fe.step(launch(e, v, d_dst, s))) return false;
+    if (ev1 && !fe.step(cudaEventRecord(ev1, s), "cudaEventRecord")) return false;
+    return dst_direct || fe.step(cudaMemcpyAsync(dst, d_dst, out_bytes, dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s), "D2H");
+}
+
 // Host surface -> host blocks for the COMPUTE-bound encoders (BC7, BC6H): the surface is cut into four row bands whose
 // H2D copies, kernels and D2H copies run on three streams, so that all but the first (small) band's input copy and all
 // but the last band's output copy hide behind the kernels.  (For BC1-BC5 the copies ARE the cost -- see encode_single.)
 // Bands are whole block rows; the kernels see each band as an independent surface, exactly as the reference's own
 // callers do (win32Threads.cpp:217-230), so the output is unchanged.
-int encode_banded(int format, const rgba_surface* src, uint8_t* dst, const void* settings, const FormatInfo& f)
+int encode_banded(const Encoder& e, const rgba_surface* src, uint8_t* dst)
 {
     ThreadCtx& c = tls;
     if (!c.copy_in) {
@@ -255,8 +314,8 @@ int encode_banded(int format, const rgba_surface* src, uint8_t* dst, const void*
             ITW_CUDA(cudaEventCreateWithFlags(&c.band_done[i], cudaEventDisableTiming));
         }
     }
-    const size_t row_bytes = (size_t)src->width * f.texel_bytes;
-    const size_t block_row_bytes = (size_t)(src->width >> 2) * f.bpb;
+    const size_t row_bytes = (size_t)src->width * e.f.texel_bytes;
+    const size_t block_row_bytes = (size_t)(src->width >> 2) * e.f.bpb;
     const int block_rows = src->height >> 2;
     if (grow(c.d_in, c.d_in_cap, row_bytes * src->height)) return -1;
     if (grow(c.d_out, c.d_out_cap, block_row_bytes * block_rows)) return -1;
@@ -274,7 +333,7 @@ int encode_banded(int format, const rgba_surface* src, uint8_t* dst, const void*
     // need as many rounds as one launch over the whole surface.
     {
         const long long bw = src->width >> 2;
-        const long long wave = (long long)c.sm_count * (format == ITW_FORMAT_BC7 ? kBc7TileBlocks : kBc6TileBlocks);
+        const long long wave = (long long)c.sm_count * (e.format == ITW_FORMAT_BC7 ? kBc7TileBlocks : kBc6TileBlocks);
         const long long total = bw * block_rows, waves = total / wave;
         if (waves >= 4 && wave >= bw) {
             const long long w0 = waves / 16 > 0 ? waves / 16 : 1;                   // waves of the first band
@@ -286,131 +345,94 @@ int encode_banded(int format, const rgba_surface* src, uint8_t* dst, const void*
             if (first[2] > first[3]) first[2] = first[3];
         }
     }
-    // Every failure after the first enqueue leaves through `drain`: async copies into the caller's dst and kernels
-    // on the three streams must not stay in flight when the call returns -1 (the caller may free src / dst).
-    int rc = 0;
-    auto step = [&](cudaError_t e, const char* what) { if (rc == 0 && e != cudaSuccess) rc = fail(what, e); return rc == 0; };
-    for (int b = 0; b < 4 && rc == 0; b++) {
+    FirstError fe;
+    for (int b = 0; b < 4; b++) {
         const int r0 = first[b], r1 = first[b + 1];
         if (r1 <= r0) continue;
         const size_t rows = (size_t)(r1 - r0) * 4;
         uint8_t* d_band = c.d_in + (size_t)r0 * 4 * row_bytes;
         const uint8_t* h_band = src->ptr + (size_t)r0 * 4 * (size_t)src->stride;
-        if ((size_t)src->stride == row_bytes) {
-            if (!step(cudaMemcpyAsync(d_band, h_band, row_bytes * rows, cudaMemcpyHostToDevice, c.copy_in), "band H2D")) break;
-        } else {
-            if (!step(cudaMemcpy2DAsync(d_band, row_bytes, h_band, (size_t)src->stride, row_bytes, rows, cudaMemcpyHostToDevice, c.copy_in), "band H2D")) break;
-        }
-        if (!step(cudaEventRecord(c.band_in[b], c.copy_in), "cudaEventRecord")) break;
-        if (!step(cudaStreamWaitEvent(c.stream, c.band_in[b], 0), "cudaStreamWaitEvent")) break;
-        if (b == 0 && !step(cudaEventRecord(c.ev0, c.stream), "cudaEventRecord")) break;
+        if (!fe.step(copy_rows_h2d(d_band, h_band, (size_t)src->stride, row_bytes, rows, c.copy_in), "band H2D")) break;
+        if (!fe.step(cudaEventRecord(c.band_in[b], c.copy_in), "cudaEventRecord")) break;
+        if (!fe.step(cudaStreamWaitEvent(c.stream, c.band_in[b], 0), "cudaStreamWaitEvent")) break;
+        if (b == 0 && !fe.step(cudaEventRecord(c.ev0, c.stream), "cudaEventRecord")) break;
         const SurfaceView v{d_band, src->width, (int)rows, (int)row_bytes};
         uint8_t* d_blocks = c.d_out + (size_t)r0 * block_row_bytes;
-        if (launch(format, v, d_blocks, settings, c.stream)) { rc = -1; break; }           // bad settings or a launch failure
-        if (!step(cudaEventRecord(c.band_done[b], c.stream), "cudaEventRecord")) break;
-        if (!step(cudaStreamWaitEvent(c.copy_out, c.band_done[b], 0), "cudaStreamWaitEvent")) break;
-        if (!step(cudaMemcpyAsync(dst + (size_t)r0 * block_row_bytes, d_blocks, (size_t)(r1 - r0) * block_row_bytes, cudaMemcpyDeviceToHost,
-                                  c.copy_out), "band D2H")) break;
+        if (!fe.step(launch(e, v, d_blocks, c.stream))) break;
+        if (!fe.step(cudaEventRecord(c.band_done[b], c.stream), "cudaEventRecord")) break;
+        if (!fe.step(cudaStreamWaitEvent(c.copy_out, c.band_done[b], 0), "cudaStreamWaitEvent")) break;
+        if (!fe.step(cudaMemcpyAsync(dst + (size_t)r0 * block_row_bytes, d_blocks, (size_t)(r1 - r0) * block_row_bytes, cudaMemcpyDeviceToHost,
+                                     c.copy_out), "band D2H")) break;
     }
-    if (rc == 0 && step(cudaEventRecord(c.ev1, c.stream), "cudaEventRecord")) c.timed = true;
-    // drain (also on error): nothing may stay in flight towards dst, and d_in / d_out must be idle for the next call
-    const cudaError_t e0 = cudaStreamSynchronize(c.copy_in), e1 = cudaStreamSynchronize(c.stream), e2 = cudaStreamSynchronize(c.copy_out);
-    if (rc == 0) { step(e0, "cudaStreamSynchronize"); step(e1, "cudaStreamSynchronize"); step(e2, "cudaStreamSynchronize"); }
-    else cudaGetLastError();
-    return rc;
+    if (fe.rc == 0 && fe.step(cudaEventRecord(c.ev1, c.stream), "cudaEventRecord")) c.timed = true;
+    return fe.drain({c.copy_in, c.stream, c.copy_out});
+}
+
+// A lane's stream exists and its staging buffers are idle (they may still be in flight from three calls ago).
+int lane_ready(ThreadCtx::Lane& L)
+{
+    if (!L.stream) ITW_CUDA(cudaStreamCreateWithFlags(&L.stream, cudaStreamNonBlocking));
+    if (L.busy) {
+        ITW_CUDA(cudaStreamSynchronize(L.stream));
+        L.busy = false;
+    }
+    return 0;
+}
+void drain_lanes(ThreadCtx& c, FirstError& fe)
+{
+    for (auto& L : c.lanes)
+        if (L.busy) {
+            fe.step(cudaStreamSynchronize(L.stream), "cudaStreamSynchronize");
+            L.busy = false;
+        }
+}
+// Device-resident operands were produced on the caller's blocking streams: order `s` after what is already enqueued on the
+// legacy default stream (the ordering rule of CompressBlocks*, see itw_bcn.h).  Uses ev0, so the call reports no kernel time.
+int order_after_legacy(cudaStream_t s)
+{
+    tls.timed = false;
+    if (cudaEventRecord(tls.ev0, cudaStreamLegacy) != cudaSuccess || cudaStreamWaitEvent(s, tls.ev0, 0) != cudaSuccess) return fail("stream ordering");
+    return 0;
 }
 
 // Deferred mode (itw_begin_deferred .. itw_flush): a host -> host encode is enqueued on one of three lanes (stream +
 // staging buffers) and the call returns; the H2D copy of call i+1 overlaps the kernel of call i and the D2H copy of call
 // i-1.  The caller keeps src and dst valid until itw_flush().  This is what makes the reference's unchanged slice loop
 // (IntelPlugin.cpp:851-879: one CompressImageMT per 256 K-texel slice) cheap: no synchronisation per slice.
-int encode_deferred(int format, const rgba_surface* src, uint8_t* dst, const void* settings, const FormatInfo& f)
+int encode_deferred(const Encoder& e, const rgba_surface* src, uint8_t* dst)
 {
     ThreadCtx& c = tls;
     ThreadCtx::Lane& L = c.lanes[c.deferred_next++ % 3];
-    if (!L.stream) ITW_CUDA(cudaStreamCreateWithFlags(&L.stream, cudaStreamNonBlocking));
-    if (L.busy) {                                      // its buffers are still in flight from three calls ago
-        ITW_CUDA(cudaStreamSynchronize(L.stream));
-        L.busy = false;
-    }
-    const size_t row_bytes = (size_t)src->width * f.texel_bytes;
-    const size_t out_bytes = (size_t)(src->width >> 2) * (src->height >> 2) * f.bpb;
-    if (grow(L.d_in, L.d_in_cap, row_bytes * src->height)) return -1;
-    if (grow(L.d_out, L.d_out_cap, out_bytes)) return -1;
-    if ((size_t)src->stride == row_bytes)
-        ITW_CUDA(cudaMemcpyAsync(L.d_in, src->ptr, row_bytes * src->height, cudaMemcpyHostToDevice, L.stream));
-    else
-        ITW_CUDA(cudaMemcpy2DAsync(L.d_in, row_bytes, src->ptr, (size_t)src->stride, row_bytes, (size_t)src->height, cudaMemcpyHostToDevice, L.stream));
+    if (lane_ready(L)) return -1;
+    FirstError fe;
     L.busy = true;
-    const SurfaceView v{L.d_in, src->width, src->height, (int)row_bytes};
-    if (launch(format, v, L.d_out, settings, L.stream)) return -1;
-    ITW_CUDA(cudaMemcpyAsync(dst, L.d_out, out_bytes, cudaMemcpyDeviceToHost, L.stream));
+    encode_surface(fe, e, src, false, dst, false, L, L.stream);
     c.timed = false;
-    return 0;
-}
-int drain_lanes(ThreadCtx& c)
-{
-    int rc = 0;
-    for (auto& L : c.lanes)
-        if (L.busy) {
-            if (cudaStreamSynchronize(L.stream) != cudaSuccess && rc == 0) rc = fail("cudaStreamSynchronize");
-            L.busy = false;
-        }
-    return rc;
+    return fe.rc;
 }
 
 // One device: src and dst may each be host or device memory.
-int encode_single(int format, const rgba_surface* src, uint8_t* dst, const void* settings, const FormatInfo& f)
+int encode_single(const Encoder& e, const rgba_surface* src, uint8_t* dst)
 {
     if (ensure_ctx()) return -1;
     ThreadCtx& c = tls;
-    // (Splitting one large host surface into pipelined row bands was measured and rejected for BC1-BC5: the H2D copy is
-    //  >90 % of the BC1 end-to-end time, so overlap buys <0.1 ms while eight smaller copies cost 0.3 ms.)
-    const size_t row_bytes = (size_t)src->width * f.texel_bytes;
-    const size_t out_bytes = (size_t)(src->width >> 2) * (src->height >> 2) * f.bpb;
     const bool src_dev = is_device_pointer(src->ptr), dst_dev = is_device_pointer(dst);
     if (!src_dev && !dst_dev && c.deferred) {
-        const int rc = encode_deferred(format, src, dst, settings, f);
+        const int rc = encode_deferred(e, src, dst);
         if (rc && c.deferred_rc == 0) c.deferred_rc = rc;
         return rc;
     }
-    if (!src_dev && !dst_dev && (format == ITW_FORMAT_BC7 || format == ITW_FORMAT_BC6H) && src->height >= 256)
-        return encode_banded(format, src, dst, settings, f);
-
+    if (!src_dev && !dst_dev && (e.format == ITW_FORMAT_BC7 || e.format == ITW_FORMAT_BC6H) && src->height >= 256)
+        return encode_banded(e, src, dst);
+    // (Splitting one large host surface into pipelined row bands was measured and rejected for BC1-BC5: the H2D copy is
+    //  >90 % of the BC1 end-to-end time, so overlap buys <0.1 ms while eight smaller copies cost 0.3 ms.)
     // Device-resident operands were produced by the caller's own streams.  The legacy default stream orders
     // after every blocking stream (torch's default stream included), which gives the synchronous call the
     // semantics a caller expects; pure host calls use this thread's private non-blocking stream.
     cudaStream_t s = (src_dev || dst_dev) ? cudaStreamLegacy : c.stream;
-    SurfaceView v{src->ptr, src->width, src->height, src->stride};
-    if (!src_dev) {                      // H2D of the tightly packed rows (pinned sources copy at PCIe rate)
-        if (grow(c.d_in, c.d_in_cap, row_bytes * src->height)) return -1;
-        if ((size_t)src->stride == row_bytes)   // tightly packed rows: one linear copy (full PCIe rate from pinned memory)
-            ITW_CUDA(cudaMemcpyAsync(c.d_in, src->ptr, row_bytes * src->height, cudaMemcpyHostToDevice, s));
-        else
-            ITW_CUDA(cudaMemcpy2DAsync(c.d_in, row_bytes, src->ptr, (size_t)src->stride, row_bytes, (size_t)src->height,
-                                       cudaMemcpyHostToDevice, s));
-        v.ptr = c.d_in;
-        v.stride = (int)row_bytes;
-    }
-    uint8_t* d_dst = dst;
-    const bool dst_ok = dst_dev && (reinterpret_cast<uintptr_t>(dst) & 15u) == 0;
-    if (!dst_ok) {
-        if (grow(c.d_out, c.d_out_cap, out_bytes)) return -1;
-        d_dst = c.d_out;
-    }
-    // From here on work is in flight on `s`: every failure still leaves through the synchronisation below (the caller may free
-    // src / dst as soon as the call returns), like encode_banded.
-    int rc = 0;
-    auto step = [&](cudaError_t e, const char* what) { if (rc == 0 && e != cudaSuccess) rc = fail(what, e); return rc == 0; };
-    step(cudaEventRecord(c.ev0, s), "cudaEventRecord");
-    if (rc == 0 && launch(format, v, d_dst, settings, s)) rc = -1;                       // bad settings or a launch failure
-    if (rc == 0 && step(cudaEventRecord(c.ev1, s), "cudaEventRecord")) c.timed = true;
-    if (rc == 0 && !dst_ok)
-        step(cudaMemcpyAsync(dst, d_dst, out_bytes, dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s), "cudaMemcpyAsync");
-    const cudaError_t e = cudaStreamSynchronize(s);
-    if (rc == 0) step(e, "cudaStreamSynchronize");
-    else cudaGetLastError();
-    return rc;
+    FirstError fe;
+    if (encode_surface(fe, e, src, src_dev, dst, dst_dev, c, s, c.ev0, c.ev1)) c.timed = true;
+    return fe.drain({s});
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -437,9 +459,9 @@ public:
     }
     int size() const { return (int)workers_.size(); }
     int device(int i) const { return workers_[i]->device; }
-    // Run jobs[i] on worker i (empty functions are skipped); returns 0 or -1 with the first error text in `err`
-    // and the largest kernel time in `ms`.
-    int run(const std::vector<std::function<int()>>& jobs, std::string& err, float& ms)
+    // Run jobs[i] on worker i (empty functions are skipped); returns 0 or -1 with the first worker's error as this thread's
+    // error.  The calling thread times no kernel of its own; `ms`, when given, receives the largest kernel time of the workers.
+    int run(const std::vector<std::function<int()>>& jobs, float* ms = nullptr)
     {
         std::lock_guard<std::mutex> serial(run_mutex_);           // concurrent callers take turns
         for (size_t i = 0; i < workers_.size() && i < jobs.size(); i++) {
@@ -449,16 +471,19 @@ public:
             w.cv.notify_all();
         }
         int rc = 0;
-        ms = -1.0f;
+        float most = -1.0f;
+        std::string err;
         for (size_t i = 0; i < workers_.size() && i < jobs.size(); i++) {
             Worker& w = *workers_[i];
             if (!jobs[i]) continue;
             std::unique_lock<std::mutex> g(w.m);
             w.cv.wait(g, [&] { return w.done; });
             if (w.rc != 0 && rc == 0) { rc = -1; err = w.err; }
-            if (w.ms > ms) ms = w.ms;
+            if (w.ms > most) most = w.ms;
         }
-        return rc;
+        tls.timed = false;
+        if (ms) *ms = most;
+        return rc ? fail(err.c_str()) : 0;
     }
 
 private:
@@ -510,14 +535,14 @@ std::shared_ptr<DevicePool> current_pool()
 // smallest band worth a device of its own: below this the per-device launch + copy latency outweighs the split
 constexpr long long kPoolMinBlocksPerDevice = 4096;
 
-int encode_fanout(DevicePool& pool, int format, const rgba_surface* src, uint8_t* dst, const void* settings, const FormatInfo& f)
+int encode_fanout(DevicePool& pool, const Encoder& e, const rgba_surface* src, uint8_t* dst)
 {
     const int block_rows = src->height >> 2;
     const long long blocks_per_row = src->width >> 2;
     int n = pool.size();
     while (n > 1 && ((long long)block_rows * blocks_per_row) / n < kPoolMinBlocksPerDevice) n--;
     if (n > block_rows) n = block_rows;
-    const size_t block_row_bytes = (size_t)blocks_per_row * f.bpb;
+    const size_t block_row_bytes = (size_t)blocks_per_row * e.f.bpb;
     std::vector<rgba_surface> bands((size_t)n);
     std::vector<std::function<int()>> jobs((size_t)pool.size());
     for (int i = 0; i < n; i++) {
@@ -525,15 +550,9 @@ int encode_fanout(DevicePool& pool, int format, const rgba_surface* src, uint8_t
         bands[i] = rgba_surface{src->ptr + (size_t)r0 * 4 * (size_t)src->stride, src->width, (r1 - r0) * 4, src->stride};
         uint8_t* out = dst + (size_t)r0 * block_row_bytes;
         const rgba_surface* band = &bands[i];
-        if (r1 > r0) jobs[i] = [=, &f]() { return encode_single(format, band, out, settings, f); };
+        if (r1 > r0) jobs[i] = [=, &e]() { return encode_single(e, band, out); };
     }
-    std::string err;
-    float ms = -1.0f;
-    const int rc = pool.run(jobs, err, ms);
-    tls.timed = false;
-    tls.pool_ms = ms;
-    if (rc) return fail(err.c_str());
-    return 0;
+    return pool.run(jobs, &tls.pool_ms);
 }
 
 // The CompressBlocks* path.
@@ -541,18 +560,22 @@ int encode_any(int format, const rgba_surface* src, uint8_t* dst, const void* se
 {
     tls.err.clear();
     tls.pool_ms = -1.0f;
-    if (format == ITW_FORMAT_BC6H_SF16) format = ITW_FORMAT_BC6H;      // one encoder for both (IntelPlugin.cpp:840-843)
     FormatInfo f;
     if (!format_info(format, f)) return fail("unknown format");
     const int chk = check_surface(src, f);
     if (chk) return chk < 0 ? -1 : 0;
     if (!dst) return fail("null dst");
+    Encoder e;
+    if (resolve_encoder(format, settings, e)) {
+        if (tls.deferred && tls.deferred_rc == 0) tls.deferred_rc = -1;      // reported again by itw_flush
+        return -1;
+    }
     if (std::shared_ptr<DevicePool> pool = current_pool()) {
         if (pool->size() > 1 && !tls.deferred && (long long)(src->width >> 2) * (src->height >> 2) >= 2 * kPoolMinBlocksPerDevice &&
             !is_device_pointer(src->ptr) && !is_device_pointer(dst))
-            return encode_fanout(*pool, format, src, dst, settings, f);
+            return encode_fanout(*pool, e, src, dst);
     }
-    return encode_single(format, src, dst, settings, f);
+    return encode_single(e, src, dst);
 }
 
 
@@ -595,32 +618,22 @@ int decode_any(int format, const uint8_t* blocks, const rgba_surface* dst)
     const size_t in_bytes = (size_t)(dst->width >> 2) * (dst->height >> 2) * f.bpb;
     const bool src_dev = is_device_pointer(blocks), dst_dev = is_device_pointer(dst->ptr);
     cudaStream_t s = (src_dev || dst_dev) ? cudaStreamLegacy : c.stream;       // same ordering rule as encode_any
-    const uint8_t* d_blocks = blocks;
-    if (!src_dev || (reinterpret_cast<uintptr_t>(blocks) & 15u)) {
-        if (grow(c.d_in, c.d_in_cap, in_bytes)) return -1;
-        ITW_CUDA(cudaMemcpyAsync(c.d_in, blocks, in_bytes, src_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
-        d_blocks = c.d_in;
-    }
-    uint8_t* d_dst = dst->ptr;
-    long long stride = dst->stride;
-    const bool dst_ok = dst_dev && (((uintptr_t)dst->ptr | (uintptr_t)dst->stride) & 3u) == 0;
-    if (!dst_ok) {
-        if (grow(c.d_out, c.d_out_cap, row_bytes * dst->height)) return -1;
-        d_dst = c.d_out;
-        stride = (long long)row_bytes;
-    }
-    int rc = 0;                                        // work is in flight from here on: every exit synchronises (see encode_single)
-    auto step = [&](cudaError_t e, const char* what) { if (rc == 0 && e != cudaSuccess) rc = fail(what, e); return rc == 0; };
-    step(cudaEventRecord(c.ev0, s), "cudaEventRecord");
-    if (rc == 0 && launch_decode(format, d_blocks, d_dst, dst->width, dst->height, stride, s)) rc = -1;
-    if (rc == 0 && step(cudaEventRecord(c.ev1, s), "cudaEventRecord")) c.timed = true;
-    if (rc == 0 && !dst_ok)
-        step(cudaMemcpy2DAsync(dst->ptr, (size_t)dst->stride, d_dst, row_bytes, row_bytes, (size_t)dst->height,
-                               dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s), "cudaMemcpy2DAsync");
-    const cudaError_t e = cudaStreamSynchronize(s);
-    if (rc == 0) step(e, "cudaStreamSynchronize");
-    else cudaGetLastError();
-    return rc;
+    const bool src_direct = src_dev && (reinterpret_cast<uintptr_t>(blocks) & 15u) == 0;
+    const bool dst_direct = dst_dev && (((uintptr_t)dst->ptr | (uintptr_t)dst->stride) & 3u) == 0;
+    if (!src_direct && grow(c.d_in, c.d_in_cap, in_bytes)) return -1;
+    if (!dst_direct && grow(c.d_out, c.d_out_cap, row_bytes * dst->height)) return -1;
+    const uint8_t* d_blocks = src_direct ? blocks : c.d_in;
+    uint8_t* d_dst = dst_direct ? dst->ptr : c.d_out;
+    const long long stride = dst_direct ? dst->stride : (long long)row_bytes;
+    FirstError fe;
+    if (!src_direct) fe.step(cudaMemcpyAsync(c.d_in, blocks, in_bytes, src_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s), "H2D");
+    if (fe.rc == 0) fe.step(cudaEventRecord(c.ev0, s), "cudaEventRecord");
+    if (fe.rc == 0) fe.step(launch_decode(format, d_blocks, d_dst, dst->width, dst->height, stride, s));
+    if (fe.rc == 0 && fe.step(cudaEventRecord(c.ev1, s), "cudaEventRecord")) c.timed = true;
+    if (fe.rc == 0 && !dst_direct)
+        fe.step(cudaMemcpy2DAsync(dst->ptr, (size_t)dst->stride, d_dst, row_bytes, row_bytes, (size_t)dst->height,
+                                  dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s), "D2H");
+    return fe.drain({s});
 }
 
 
@@ -631,6 +644,7 @@ int front_params(FrontParams& P, int format, const itw_pixel_source* src, uint32
     if (!format_info(format, f)) return fail("unknown format");
     if (!src || !src->data) return fail("null pixel source");
     if (src->width <= 0 || src->height <= 0) return fail("pixel source: width/height must be positive");
+    if (pad4(src->height) > 65535) return fail("pixel source: height above 65532");      // one grid row per (padded) output row
     if (src->planes < 1 || src->planes > 4) return fail("pixel source: planes must be 1..4");
     if (src->depth != 8 && src->depth != 16 && src->depth != 32) return fail("pixel source: depth must be 8, 16 or 32");
     if (flags & ~31u) return fail("unknown front-end flag");
@@ -660,7 +674,6 @@ void launch_front_x4(const FrontParams& P, dim3 grid, cudaStream_t s, uint8_t* d
 }
 int launch_front(const FrontParams& P, uint8_t* d_dst, int dw, int dh, long long dstride, cudaStream_t s)
 {
-    if (dh > 65535) return fail("front end: height above 65535");
     const bool quads = (dw & 3) == 0 && ((reinterpret_cast<uintptr_t>(d_dst) | (uintptr_t)dstride) & 15u) == 0 &&
                        ((reinterpret_cast<uintptr_t>(P.data) | (uintptr_t)P.row_bytes) & 3u) == 0;
     if (quads) {
@@ -676,13 +689,13 @@ int launch_front(const FrontParams& P, uint8_t* d_dst, int dw, int dh, long long
     ITW_CUDA(cudaGetLastError());
     return 0;
 }
-// Stage a host pixel source in d_in (tight rows); P.data / P.row_bytes are redirected.
-int stage_pixels(ThreadCtx& c, FrontParams& P, cudaStream_t s)
+// Stage a host pixel source in `buf` (tight rows); P.data / P.row_bytes are redirected.
+int stage_pixels(uint8_t*& buf, size_t& cap, FrontParams& P, cudaStream_t s)
 {
     const size_t tight = (size_t)P.width * P.planes * (P.depth / 8);
-    if (grow(c.d_in, c.d_in_cap, tight * P.height)) return -1;
-    ITW_CUDA(cudaMemcpy2DAsync(c.d_in, tight, P.data, (size_t)P.row_bytes, tight, (size_t)P.height, cudaMemcpyHostToDevice, s));
-    P.data = c.d_in;
+    if (grow(buf, cap, tight * P.height)) return -1;
+    ITW_CUDA(copy_rows_h2d(buf, P.data, (size_t)P.row_bytes, tight, (size_t)P.height, s));
+    P.data = buf;
     P.row_bytes = (long long)tight;
     return 0;
 }
@@ -693,33 +706,26 @@ int convert_any(int format, const itw_pixel_source* src, uint32_t flags, const r
     if (front_params(P, format, src, flags)) return -1;
     if (!dst || !dst->ptr) return fail("null surface");
     const int texel = (P.family == 2) ? 8 : 4;
-    const int pw = (P.width + 3) & ~3, ph = (P.height + 3) & ~3;
-    if (!((dst->width == P.width && dst->height == P.height) || (dst->width == pw && dst->height == ph)))
+    if (!((dst->width == P.width && dst->height == P.height) || (dst->width == pad4(P.width) && dst->height == pad4(P.height))))
         return fail("itw_convert_pixels: dst must have the source size or that size rounded up to multiples of 4");
     if ((long long)dst->stride < (long long)dst->width * texel) return fail("surface stride smaller than a texel row");
     if (ensure_ctx()) return -1;
     ThreadCtx& c = tls;
     const bool src_dev = is_device_pointer(P.data), dst_dev = is_device_pointer(dst->ptr);
     cudaStream_t s = (src_dev || dst_dev) ? cudaStreamLegacy : c.stream;
-    if (!src_dev && stage_pixels(c, P, s)) return -1;
-    uint8_t* d_dst = dst->ptr;
-    long long stride = dst->stride;
-    const bool dst_ok = dst_dev && (((uintptr_t)dst->ptr | (uintptr_t)dst->stride) & (uintptr_t)(texel - 1)) == 0;
+    const bool dst_direct = dst_dev && (((uintptr_t)dst->ptr | (uintptr_t)dst->stride) & (uintptr_t)(texel - 1)) == 0;
     const size_t row_bytes = (size_t)dst->width * texel;
-    if (!dst_ok) {
-        if (grow(c.d_out, c.d_out_cap, row_bytes * dst->height)) return -1;
-        d_dst = c.d_out;
-        stride = (long long)row_bytes;
-    }
-    ITW_CUDA(cudaEventRecord(c.ev0, s));
-    if (launch_front(P, d_dst, dst->width, dst->height, stride, s)) return -1;
-    ITW_CUDA(cudaEventRecord(c.ev1, s));
-    c.timed = true;
-    if (!dst_ok)
-        ITW_CUDA(cudaMemcpy2DAsync(dst->ptr, (size_t)dst->stride, d_dst, row_bytes, row_bytes, (size_t)dst->height,
-                                   dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s));
-    ITW_CUDA(cudaStreamSynchronize(s));
-    return 0;
+    if (!dst_direct && grow(c.d_out, c.d_out_cap, row_bytes * dst->height)) return -1;
+    uint8_t* d_dst = dst_direct ? dst->ptr : c.d_out;
+    FirstError fe;
+    if (!src_dev) fe.step(stage_pixels(c.d_in, c.d_in_cap, P, s));
+    if (fe.rc == 0) fe.step(cudaEventRecord(c.ev0, s), "cudaEventRecord");
+    if (fe.rc == 0) fe.step(launch_front(P, d_dst, dst->width, dst->height, dst_direct ? dst->stride : (long long)row_bytes, s));
+    if (fe.rc == 0 && fe.step(cudaEventRecord(c.ev1, s), "cudaEventRecord")) c.timed = true;
+    if (fe.rc == 0 && !dst_direct)
+        fe.step(cudaMemcpy2DAsync(dst->ptr, (size_t)dst->stride, d_dst, row_bytes, row_bytes, (size_t)dst->height,
+                                  dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s), "D2H");
+    return fe.drain({s});
 }
 // convert + pad + encode; the intermediate surface never leaves the GPU
 int encode_pixels_any(int format, const itw_pixel_source* src, uint32_t flags, const void* settings, uint8_t* dst)
@@ -728,32 +734,22 @@ int encode_pixels_any(int format, const itw_pixel_source* src, uint32_t flags, c
     FrontParams P;
     if (front_params(P, format, src, flags)) return -1;
     if (!dst) return fail("null dst");
-    FormatInfo f;
-    format_info(format, f);
+    Encoder e;
+    if (resolve_encoder(format, settings, e)) return -1;
     if (ensure_ctx()) return -1;
     ThreadCtx& c = tls;
-    const int pw = (P.width + 3) & ~3, ph = (P.height + 3) & ~3;
-    const size_t mid_row = (size_t)pw * f.texel_bytes, out_bytes = (size_t)(pw >> 2) * (ph >> 2) * f.bpb;
+    const int pw = pad4(P.width), ph = pad4(P.height);
+    const size_t mid_row = (size_t)pw * e.f.texel_bytes;
+    if (grow(c.d_mid, c.d_mid_cap, mid_row * ph)) return -1;
     const bool src_dev = is_device_pointer(P.data), dst_dev = is_device_pointer(dst);
     cudaStream_t s = (src_dev || dst_dev) ? cudaStreamLegacy : c.stream;
-    if (!src_dev && stage_pixels(c, P, s)) return -1;
-    if (grow(c.d_mid, c.d_mid_cap, mid_row * ph)) return -1;
-    uint8_t* d_dst = dst;
-    const bool dst_ok = dst_dev && (reinterpret_cast<uintptr_t>(dst) & 15u) == 0;
-    if (!dst_ok) {
-        if (grow(c.d_out, c.d_out_cap, out_bytes)) return -1;
-        d_dst = c.d_out;
-    }
-    ITW_CUDA(cudaEventRecord(c.ev0, s));
-    if (launch_front(P, c.d_mid, pw, ph, (long long)mid_row, s)) return -1;
-    const SurfaceView v{c.d_mid, pw, ph, (int)mid_row};
-    if (launch(format, v, d_dst, settings, s)) return -1;
-    ITW_CUDA(cudaEventRecord(c.ev1, s));
-    c.timed = true;
-    if (!dst_ok)
-        ITW_CUDA(cudaMemcpyAsync(dst, d_dst, out_bytes, dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s));
-    ITW_CUDA(cudaStreamSynchronize(s));
-    return 0;
+    const rgba_surface mid{c.d_mid, pw, ph, (int)mid_row};
+    FirstError fe;
+    if (!src_dev) fe.step(stage_pixels(c.d_in, c.d_in_cap, P, s));
+    if (fe.rc == 0) fe.step(cudaEventRecord(c.ev0, s), "cudaEventRecord");
+    if (fe.rc == 0) fe.step(launch_front(P, c.d_mid, pw, ph, (long long)mid_row, s));
+    if (fe.rc == 0 && encode_surface(fe, e, &mid, true, dst, dst_dev, c, s, nullptr, c.ev1)) c.timed = true;
+    return fe.drain({s});
 }
 
 }  // namespace
@@ -801,10 +797,12 @@ int itw_encode_device(int format, const rgba_surface* src, uint8_t* dst, const v
     if (const int chk = check_surface(src, f)) return chk < 0 ? -1 : 0;
     if (!dst) return fail("null dst");
     if (reinterpret_cast<uintptr_t>(dst) & 15u) return fail("itw_encode_device: dst must be 16-byte aligned");
+    Encoder e;
+    if (resolve_encoder(format, settings, e)) return -1;
     if (ensure_ctx()) return -1;
     tls.timed = false;
     SurfaceView v{src->ptr, src->width, src->height, src->stride};
-    return launch(format, v, dst, settings, static_cast<cudaStream_t>(cuda_stream));
+    return launch(e, v, dst, static_cast<cudaStream_t>(cuda_stream));
 }
 
 int itw_decode(int format, const uint8_t* blocks, const rgba_surface* dst) { return decode_any(format, blocks, dst); }
@@ -824,76 +822,40 @@ int itw_encode_batch(int format, const rgba_surface* srcs, uint8_t* const* dsts,
 
 namespace {
 // Tiles i = first, first+step, ... of the batch on THIS thread's device, pipelined over the three lanes.
-int encode_many_single(int format, const rgba_surface* srcs, uint8_t* const* dsts, int count, const void* settings, int first, int step)
+int encode_many_single(const Encoder& e, const rgba_surface* srcs, uint8_t* const* dsts, int count, int first, int step)
 {
-    FormatInfo f;
-    if (!format_info(format, f)) return fail("unknown format");
     if (ensure_ctx()) return -1;
     ThreadCtx& c = tls;
-    int rc = drain_lanes(c);
-    // Device-resident operands were produced by the caller's blocking streams: make every lane wait for what is already
-    // enqueued on the legacy default stream (the ordering rule of CompressBlocks*, see itw_bcn.h), once per call.
-    bool any_dev = false;
+    FirstError fe;
+    drain_lanes(c, fe);
+    bool any_dev = false;                                // then every lane waits for the caller's streams, once per call
     for (int i = first; i < count && !any_dev; i += step) any_dev = is_device_pointer(srcs[i].ptr) || is_device_pointer(dsts[i]);
-    if (any_dev && rc == 0) {
-        if (cudaEventRecord(c.ev0, cudaStreamLegacy) != cudaSuccess) rc = fail("cudaEventRecord");
-        for (auto& L : c.lanes) {
-            if (rc) break;
-            if (!L.stream && cudaStreamCreateWithFlags(&L.stream, cudaStreamNonBlocking) != cudaSuccess) { rc = fail("cudaStreamCreate"); break; }
-            if (cudaStreamWaitEvent(L.stream, c.ev0, 0) != cudaSuccess) rc = fail("cudaStreamWaitEvent");
-        }
-    }
+    if (any_dev)
+        for (auto& L : c.lanes)
+            if (!fe.step(lane_ready(L)) || !fe.step(order_after_legacy(L.stream))) break;
     unsigned turn = 0;
-    for (int i = first; i < count && rc == 0; i += step) {
-        const rgba_surface* src = &srcs[i];
-        uint8_t* dst = dsts[i];
-        const int chk = check_surface(src, f);
-        if (chk < 0) { rc = -1; break; }
-        if (chk > 0) continue;
-        if (!dst) { rc = fail("null dst"); break; }
+    for (int i = first; i < count && fe.rc == 0; i += step) {
+        if (srcs[i].height == 0) continue;                 // zero-height tiles: nothing to do (check_surface)
         ThreadCtx::Lane& L = c.lanes[turn++ % 3];
-        if (!L.stream && cudaStreamCreateWithFlags(&L.stream, cudaStreamNonBlocking) != cudaSuccess) { rc = fail("cudaStreamCreate"); break; }
-        if (L.busy) {                                  // its buffers are still in flight from three tiles ago
-            if (cudaStreamSynchronize(L.stream) != cudaSuccess) { rc = fail("cudaStreamSynchronize"); break; }
-            L.busy = false;
-        }
-        const size_t row_bytes = (size_t)src->width * f.texel_bytes;
-        const size_t out_bytes = (size_t)(src->width >> 2) * (src->height >> 2) * f.bpb;
-        const bool src_dev = is_device_pointer(src->ptr), dst_dev = is_device_pointer(dst);
-        SurfaceView v{src->ptr, src->width, src->height, src->stride};
-        cudaError_t e = cudaSuccess;
-        if (!src_dev) {
-            if (grow(L.d_in, L.d_in_cap, row_bytes * src->height)) { rc = -1; break; }
-            if ((size_t)src->stride == row_bytes)
-                e = cudaMemcpyAsync(L.d_in, src->ptr, row_bytes * src->height, cudaMemcpyHostToDevice, L.stream);
-            else
-                e = cudaMemcpy2DAsync(L.d_in, row_bytes, src->ptr, (size_t)src->stride, row_bytes, (size_t)src->height,
-                                      cudaMemcpyHostToDevice, L.stream);
-            if (e != cudaSuccess) { rc = fail("itw_encode_batch H2D", e); break; }
-            v.ptr = L.d_in;
-            v.stride = (int)row_bytes;
-        }
-        uint8_t* d_dst = dst;
-        const bool dst_ok = dst_dev && (reinterpret_cast<uintptr_t>(dst) & 15u) == 0;
-        if (!dst_ok) {
-            if (grow(L.d_out, L.d_out_cap, out_bytes)) { rc = -1; break; }
-            d_dst = L.d_out;
-        }
+        if (!fe.step(lane_ready(L))) break;
         L.busy = true;
-        if (launch(format, v, d_dst, settings, L.stream)) { rc = -1; break; }
-        if (!dst_ok) {
-            e = cudaMemcpyAsync(dst, d_dst, out_bytes, dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, L.stream);
-            if (e != cudaSuccess) { rc = fail("itw_encode_batch D2H", e); break; }
-        }
+        encode_surface(fe, e, &srcs[i], is_device_pointer(srcs[i].ptr), dsts[i], is_device_pointer(dsts[i]), L, L.stream);
     }
-    if (drain_lanes(c) && rc == 0) rc = -1;               // always drain, also on error
+    drain_lanes(c, fe);
     tls.timed = false;
-    return rc;
+    return fe.rc;
 }
 int encode_many(int format, const rgba_surface* srcs, uint8_t* const* dsts, int count, const void* settings)
 {
     tls.pool_ms = -1.0f;
     if (count < 0 || (count > 0 && (!srcs || !dsts))) return fail("itw_encode_batch: bad arguments");
+    Encoder e;
+    if (resolve_encoder(format, settings, e)) return -1;
+    for (int i = 0; i < count; i++) {
+        const int chk = check_surface(&srcs[i], e.f);
+        if (chk < 0) return -1;
+        if (chk == 0 && !dsts[i]) return fail("null dst");
+    }
     // tile stream over several devices (SURVEY.md 8e, config C5): host tiles are dealt round-robin, every device runs its
     // own three-lane pipeline; no collective
     if (std::shared_ptr<DevicePool> pool = current_pool()) {
@@ -903,16 +865,11 @@ int encode_many(int format, const rgba_surface* srcs, uint8_t* const* dsts, int 
         if (host_only) {
             const int n = pool->size() < count ? pool->size() : count;
             std::vector<std::function<int()>> jobs((size_t)pool->size());
-            for (int k = 0; k < n; k++) jobs[k] = [=]() { return encode_many_single(format, srcs, dsts, count, settings, k, n); };
-            std::string err;
-            float ms = -1.0f;
-            const int rc = pool->run(jobs, err, ms);
-            tls.timed = false;
-            if (rc) return fail(err.c_str());
-            return 0;
+            for (int k = 0; k < n; k++) jobs[k] = [=, &e]() { return encode_many_single(e, srcs, dsts, count, k, n); };
+            return pool->run(jobs);
         }
     }
-    return encode_many_single(format, srcs, dsts, count, settings, 0, 1);
+    return encode_many_single(e, srcs, dsts, count, 0, 1);
 }
 }  // namespace
 
@@ -971,13 +928,11 @@ int itw_begin_deferred(void)
 int itw_flush(void)
 {
     ThreadCtx& c = tls;
-    int rc = c.deferred_rc;
-    const std::string first = c.err;                      // the first failure of a deferred call is the one reported
-    if (drain_lanes(c) && rc == 0) rc = -1;
-    else if (rc) c.err = first;
+    FirstError fe{c.deferred_rc};                         // the first failure of a deferred call is the one reported
+    drain_lanes(c, fe);
     c.deferred = false;
     c.deferred_rc = 0;
-    return rc;
+    return fe.rc;
 }
 
 // ---- the reference's coarse seam (3rdParty/Intel/Source/win32Threads.h:24, :52-80; win32Threads.cpp:192-330) ----
