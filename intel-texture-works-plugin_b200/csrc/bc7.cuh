@@ -7,8 +7,10 @@
 // The 32 lanes are spread over the blocks' independent work items instead of over texels:
 //   * shape phases: a shape's error is the sum of its subsets' errors, and a subset's fit, endpoints and error depend on its
 //     texel mask alone (the reference refits per shape and mode, K:1279-1297, with identical results).  So the three-subset
-//     shapes go lane <-> (block, distinct mask): fit once, quantise for modes 0 and 2 and search for mode 2, then lane <->
-//     (block, shape) adds three stored mode-2 errors and searches mode 0 from the stored endpoints.  A two-subset shape
+//     shapes go lane <-> (block, two distinct masks) over the four blocks of a group: one routine fits both masks
+//     (bc7_fit_masks2: two moment passes, two independent power iterations, one projection loop), quantises them for modes 0
+//     and 2, and one walk over both masks' texels searches them for mode 2; then lane <-> (block, shape) adds three stored
+//     mode-2 errors and searches mode 0 from the stored endpoints.  A two-subset shape
 //     (modes 1, 3, 7) belongs to one lane.  When the profile searches all 64 of them for modes 1 / 3, lane <-> (block, shape)
 //     over the four blocks of a group: one routine fits both subsets (bc7_fit_pair: subset 1's moments are the block's minus
 //     subset 0's, two independent power iterations, one projection loop) and gives the split keys, and one walk over the 16
@@ -99,11 +101,11 @@ struct Bc7Warp {
     u32 palette[40][32];                       // lane-private scratch of the index search, [entry][lane]: 24 palette
                                                // entries, then 5 per-subset constants x 3 subsets
     union {
-        // every DISTINCT three-subset mask, for the two blocks being processed (bc7_phase_masks3 -> bc7_phase_shapes3): the
+        // every DISTINCT three-subset mask, for the four blocks of the group (bc7_phase_masks3 -> bc7_phase_shapes3): the
         // mode-2 subset error of all 140 masks, the decoded mode-0 endpoints (A, B as RGBA bytes) of the 36 masks of shapes 0..15
         struct {
-            int err2[2][ITW_MASK3_COUNT];
-            u32 ends0[2][ITW_MASK3_FIRST][2];
+            int err2[kBc7Slots][ITW_MASK3_COUNT];
+            u32 ends0[kBc7Slots][ITW_MASK3_FIRST][2];
         } masks3;
         // two-subset shapes of the group, after its three-subset phases
         struct {
@@ -420,6 +422,65 @@ ITW_HD_NOINLINE Bc7Pair bc7_fit_pair(const Bc7Block* blk, u32 mask0, int channel
     else bc7_fit_pair_impl<3, true>(f, blk, mask0);
     return f;
 }
+// Two subset masks of an untransformed block at three channels (a lane pair of the three-subset masks): the same values as
+// bc7_fit(blk, 3, 1, mask, 3) of each.  The masks are not complements, so each has its own moment pass; the two covariance /
+// power-iteration chains are independent, so the scheduler can interleave them; one projection loop converts every texel
+// once and projects it onto both axes.  Inlined into bc7_phase_masks3, like bc7_masks_error2: as non-inlined routines they
+// moved ptxas's register assignment of the shared callees so that bc7_chain spilled 160 bytes instead of 4 to 20
+// (-Xptxas -v), and basic / alpha_basic ran 0.4 / 1.4 % slower on H100.
+struct Bc7Segs2 { Bc7Seg seg[2]; };
+ITW_HD Bc7Segs2 bc7_fit_masks2(const Bc7Block* blk, u32 mask_a, u32 mask_b)
+{
+    u32 P[4][4];
+    load_planes(P, View{blk, 3, 1});
+    int sta[15], stb[15];
+    moments_u8(sta, P, mask_a, 3);
+    moments_u8(stb, P, mask_b, 3);
+    float cova[10], covb[10], meana[4], meanb[4];
+    bc7_covariance<3>(cova, meana, sta);
+    bc7_covariance<3>(covb, meanb, stb);
+    const float inv_var = 1.0f / (256.0f * 256.0f);
+#pragma unroll
+    for (int i = 0; i < 10; i++) { cova[i] *= inv_var; covb[i] *= inv_var; }
+    const float eps = 0.001f * 0.001f;
+    cova[0] += eps; cova[4] += eps; cova[7] += eps; cova[9] += eps;
+    covb[0] += eps; covb[4] += eps; covb[7] += eps; covb[9] += eps;
+    float axisa[4] = {1.0f, 1.0f, 1.0f, 1.0f}, axisb[4] = {1.0f, 1.0f, 1.0f, 1.0f};
+    bc7_power_axis<3, 4>(axisa, cova);
+    bc7_power_axis<3, 4>(axisb, covb);
+    bc7_power_axis<3, 4>(axisa, cova);
+    bc7_power_axis<3, 4>(axisb, covb);
+
+    float loa = inf_f(), hia = -inf_f(), lob = inf_f(), hib = -inf_f();
+#pragma unroll
+    for (int k = 0; k < 16; k++) {
+        // bc7_fit_impl's projection onto each mask's axis and mean: same operands, same order
+        float x[3];
+#pragma unroll
+        for (int c = 0; c < 3; c++) x[c] = (float)((P[c][k >> 2] >> (8 * (k & 3))) & 255u);
+        float da = axisa[0] * (x[0] - meana[0]), db = axisb[0] * (x[0] - meanb[0]);
+#pragma unroll
+        for (int c = 1; c < 3; c++) {
+            da += axisa[c] * (x[c] - meana[c]);
+            db += axisb[c] * (x[c] - meanb[c]);
+        }
+        if ((mask_a >> k) & 1u) { loa = fminf(loa, da); hia = fmaxf(hia, da); }
+        if ((mask_b >> k) & 1u) { lob = fminf(lob, db); hib = fmaxf(hib, db); }
+    }
+    if (hia - loa < 1.0f) { loa -= 0.5f; hia += 0.5f; }
+    if (hib - lob < 1.0f) { lob -= 0.5f; hib += 0.5f; }
+    Bc7Segs2 f;
+#pragma unroll
+    for (int i = 0; i < 8; i++) f.seg[0].v[i] = f.seg[1].v[i] = 0.0f;
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        f.seg[0].v[c] = clamp_sse(loa * axisa[c] + meana[c], 0.0f, 255.0f);
+        f.seg[0].v[4 + c] = clamp_sse(hia * axisa[c] + meana[c], 0.0f, 255.0f);
+        f.seg[1].v[c] = clamp_sse(lob * axisb[c] + meanb[c], 0.0f, 255.0f);
+        f.seg[1].v[4 + c] = clamp_sse(hib * axisb[c] + meanb[c], 0.0f, 255.0f);
+    }
+    return f;
+}
 
 // trace - lambda_max of a covariance; K:907-939 (eps on three diagonal slots only, K:918-920)
 template <int CH>
@@ -727,22 +788,32 @@ ITW_HD int bc7_texel_error3(const Bc7Sub3& s, u32 t)
     const u32 d0 = absdiff_u8x4(lo, t), d1 = absdiff_u8x4(hi, t);
     return mini((int)dp4a_u8(d0, d0, 0u), (int)dp4a_u8(d1, d1, 0u));
 }
-// Mode-2 error of ONE subset mask: a subset's endpoints depend on its mask alone, so the three-subset phases search every
-// distinct mask once.  A counted loop over the set bits, unrolled so that the texel loads of several iterations are in
-// flight at once (a rolled loop waits for each load: four warps per scheduler do not hide that latency).
-ITW_HD_NOINLINE int bc7_subset_error(const Bc7Block* blk, u32 mask, u32 dec_a, u32 dec_b)
+// Mode-2 errors of the two subset masks of a lane pair: a subset's endpoints depend on its mask alone, so the three-subset
+// phases search every distinct mask once.  One counted loop walks the set bits of both masks, so that the two error chains
+// interleave; it is unrolled so that the texel loads of several iterations are in flight at once (a rolled loop waits for
+// each load: four warps per scheduler do not hide that latency).  Each mask uses its own constants (e*a, e*b = decoded
+// endpoints A, B).
+struct Bc7Err2 { int a, b; };
+ITW_HD Bc7Err2 bc7_masks_error2(const Bc7Block* blk, u32 mask_a, u32 mask_b, u32 ea_a, u32 ea_b, u32 eb_a, u32 eb_b)
 {
-    const Bc7Sub2 s = bc7_sub2(dec_a, dec_b);
-    const int n = popcount16(mask);
-    int total = 0;
-    u32 rest = mask;
+    const Bc7Sub2 sa = bc7_sub2(ea_a, ea_b), sb = bc7_sub2(eb_a, eb_b);
+    const int n = mini(popcount16(mask_a), popcount16(mask_b));
+    int ta = 0, tb = 0;
+    u32 ra = mask_a, rb = mask_b;
 #pragma unroll 4
     for (int i = 0; i < n; i++) {
-        const u32 low = rest & (0u - rest);
-        rest ^= low;
-        total += bc7_texel_error2(s, blk->rgb[popcount32(low - 1u)]);
+        const u32 la = ra & (0u - ra), lb = rb & (0u - rb);
+        ra ^= la;
+        rb ^= lb;
+        ta += bc7_texel_error2(sa, blk->rgb[popcount32(la - 1u)]);
+        tb += bc7_texel_error2(sb, blk->rgb[popcount32(lb - 1u)]);
     }
-    return total;
+    // the rest of the longer mask: only one pair of the table has unequal popcounts (tools/gen_mask_tables.py)
+#pragma unroll 1
+    for (; ra; ra &= ra - 1u) ta += bc7_texel_error2(sa, blk->rgb[popcount32((ra & (0u - ra)) - 1u)]);
+#pragma unroll 1
+    for (; rb; rb &= rb - 1u) tb += bc7_texel_error2(sb, blk->rgb[popcount32((rb & (0u - rb)) - 1u)]);
+    return Bc7Err2{ta, tb};
 }
 // Mode-1 (three-bit) and mode-3 (two-bit) errors of one two-subset shape, mask0 = its subset 0: one walk over the 16 texels,
 // each scored against its own subset's constants.  e1 / e3 = decoded endpoints A, B of subsets 0 and 1 for mode 1 / mode 3.
@@ -1261,48 +1332,59 @@ ITW_HD_NOINLINE void bc7_eval_shape(Bc7Warp& W, int lane, int slot, const Bc7Blo
 // ---- three-subset shapes (modes 0 and 2) -------------------------------------------------------------------
 // The 64 shapes x 3 subsets use only 140 distinct texel masks, and the PCA fit, the endpoint quantisation and the index-search
 // error of a subset depend on its mask alone (the reference refits per shape and per mode with identical results,
-// K:1279-1297).  So, two blocks at a time (`duo` = 0..3: blocks 2*duo, 2*duo+1 of the batch): phase A fits and quantises
-// every distinct mask once and searches it for mode 2 (lane <-> (block, mask)); phase B adds up the mode-2 errors of every
-// shape's three masks and runs the mode-0 search of shapes 0..15 from the stored endpoints (lane <-> (block, shape)).  Same
-// values as evaluating shape by shape: 25 % fewer fits and quantisations, 27 % fewer mode-2 texels searched.  Mode 0 stays
-// per shape: its 72 masks of two blocks take three passes of short, divergent subset loops where its 32 shapes take one
-// dense pass, and that measured slower on the profiles that skip mode 2 (basic).
-ITW_HD void bc7_phase_masks3(int lane, Bc7Warp& W, const Bc7Params& P, int duo)
+// K:1279-1297).  So, for the four blocks of group g: phase A fits and quantises every distinct mask once and searches it for
+// mode 2, two masks of one block per lane (lane <-> (block, lane pair of itw_masks3.cuh): bc7_fit_masks2 and
+// bc7_masks_error2 run two independent chains each); phase B adds up the mode-2 errors of every shape's three masks and
+// runs the mode-0 search of shapes 0..15 from the stored endpoints (lane <-> (block, shape)).  Same values as evaluating
+// shape by shape: 25 % fewer fits and quantisations, 27 % fewer mode-2 texels searched.  Mode 0 stays per shape: its 36
+// masks per block take several passes of short, divergent subset loops where its 16 shapes per block fill a dense pass, and
+// that measured slower on the profiles that skip mode 2 (basic).
+ITW_HD void bc7_phase_masks3(int lane, Bc7Warp& W, const Bc7Params& P, int g)
 {
     const int ca = bc7_slot_count(P, 0), cb = bc7_slot_count(P, 1);
-    const int nmask = (cb > 0) ? ITW_MASK3_COUNT : ITW_MASK3_FIRST;
-    const int nslots = mini(maxi(W.nvalid - 2 * duo, 0), 2);
-    for (int t = lane; t < nslots * nmask; t += 32) {
-        // the two blocks alternate, so that a step holds 16 masks of similar popcount
-        const int s = (nslots == 2) ? (t & 1) : 0, u = (nslots == 2) ? (t >> 1) : t;
-        const Bc7Block* blk = &W.blk[2 * duo + s];
-        const u32 mask = ITW_TABLE(mask3_unique)[u];
-        const Bc7Seg seg = bc7_fit(blk, 3, 1, mask, 3);
-        if (cb > 0) {
-            const Bc7Packed pk = bc7_quantise(seg, 2, 3);
-            W.masks3.err2[s][u] = bc7_subset_error(blk, mask, pk.dec_a, pk.dec_b);
+    const int npairs = ((cb > 0) ? ITW_MASK3_COUNT : ITW_MASK3_FIRST) / 2;
+    const int nv = bc7_group_count(W, g);
+    for (int t = lane; t < nv * npairs; t += 32) {
+        // the blocks alternate, so that a step holds eight lane pairs of similar popcount
+        const int slot = t % nv, u = 2 * (t / nv);
+        const Bc7Block* blk = &W.blk[kBc7Slots * g + slot];
+        const u32 mask_a = ITW_TABLE(mask3_unique)[u], mask_b = ITW_TABLE(mask3_unique)[u + 1];
+        const Bc7Segs2 f = bc7_fit_masks2(blk, mask_a, mask_b);
+        // every quantisation before the search, so that the two fits are dead across it
+        if (ca > 0 && u < ITW_MASK3_FIRST) {                       // ITW_MASK3_FIRST is even: both masks or neither
+#pragma unroll
+            for (int j = 0; j < 2; j++) {
+                const Bc7Packed pk = bc7_quantise(f.seg[j], 0, 3);
+                W.masks3.ends0[slot][u + j][0] = pk.dec_a;
+                W.masks3.ends0[slot][u + j][1] = pk.dec_b;
+            }
         }
-        if (ca > 0 && u < ITW_MASK3_FIRST) {
-            const Bc7Packed pk = bc7_quantise(seg, 0, 3);
-            W.masks3.ends0[s][u][0] = pk.dec_a;
-            W.masks3.ends0[s][u][1] = pk.dec_b;
+        if (cb > 0) {
+            const Bc7Packed pa = bc7_quantise(f.seg[0], 2, 3), pb = bc7_quantise(f.seg[1], 2, 3);
+            const Bc7Err2 e = bc7_masks_error2(blk, mask_a, mask_b, pa.dec_a, pa.dec_b, pb.dec_a, pb.dec_b);
+            W.masks3.err2[slot][u] = e.a;
+            W.masks3.err2[slot][u + 1] = e.b;
         }
     }
 }
-ITW_HD void bc7_phase_shapes3(int lane, Bc7Warp& W, const Bc7Params& P, int duo)
+// Tasks [0, nv * ca) are block-major (slot, shape n < ca): the mode-0 searches fill whole steps; the tasks after them only add
+// up the mode-2 errors of shapes [ca, cb).
+ITW_HD void bc7_phase_shapes3(int lane, Bc7Warp& W, const Bc7Params& P, int g)
 {
     const int ca = bc7_slot_count(P, 0), cb = bc7_slot_count(P, 1);
-    const int count = maxi(ca, cb);
-    const int nslots = mini(maxi(W.nvalid - 2 * duo, 0), 2);
-    for (int t = lane; t < nslots * count; t += 32) {
-        const int s = t / count, n = t - s * count;
-        const int slot = (2 * duo + s) & (kBc7Slots - 1);             // scratch index inside the group
+    const int nv = bc7_group_count(W, g);
+    const int nfirst = nv * ca, rest = maxi(cb - ca, 0);
+    for (int t = lane; t < nfirst + nv * rest; t += 32) {
+        int slot, n;
+        if (t < nfirst) { slot = t / ca; n = t - slot * ca; }
+        else { const int u = t - nfirst; slot = u / rest; n = ca + (u - slot * rest); }
         const int u0 = ITW_TABLE(shape3_mask_id)[3 * n], u1 = ITW_TABLE(shape3_mask_id)[3 * n + 1], u2 = ITW_TABLE(shape3_mask_id)[3 * n + 2];
-        const u32 (&e)[ITW_MASK3_FIRST][2] = W.masks3.ends0[s];
-        if (n < ca)
-            W.cand_err[slot][0][n] = bc7_assign(W.palette, lane, &W.blk[2 * duo + s], 3, 1, 3, 3, shape_pattern(64 + n), e[u0][0], e[u0][1],
-                                                e[u1][0], e[u1][1], e[u2][0], e[u2][1], 0x00FFFFFFu).err;
-        if (n < cb) W.cand_err[slot][1][n] = W.masks3.err2[s][u0] + W.masks3.err2[s][u1] + W.masks3.err2[s][u2];
+        if (n < ca) {
+            const u32 (&e)[ITW_MASK3_FIRST][2] = W.masks3.ends0[slot];
+            W.cand_err[slot][0][n] = bc7_assign(W.palette, lane, &W.blk[kBc7Slots * g + slot], 3, 1, 3, 3, shape_pattern(64 + n), e[u0][0],
+                                                e[u0][1], e[u1][0], e[u1][1], e[u2][0], e[u2][1], 0x00FFFFFFu).err;
+        }
+        if (n < cb) W.cand_err[slot][1][n] = W.masks3.err2[slot][u0] + W.masks3.err2[slot][u1] + W.masks3.err2[slot][u2];
     }
 }
 
@@ -1443,10 +1525,8 @@ ITW_HD void bc7_phase_store(int lane, Bc7Warp& W, const Bc7Params& P, uint8_t* d
 // `out_block` of `dst`), as a list of (phase, barrier) pairs.
 #define ITW_BC7_GROUP_PROGRAM(PHASE, g)                                                \
     if (P.sel[0]) {                                                                    \
-        PHASE(bc7_phase_masks3(lane, W, P, 2 * (g)));                                  \
-        PHASE(bc7_phase_shapes3(lane, W, P, 2 * (g)));                                 \
-        PHASE(bc7_phase_masks3(lane, W, P, 2 * (g) + 1));                              \
-        PHASE(bc7_phase_shapes3(lane, W, P, 2 * (g) + 1));                             \
+        PHASE(bc7_phase_masks3(lane, W, P, g));                                        \
+        PHASE(bc7_phase_shapes3(lane, W, P, g));                                       \
         PHASE(bc7_phase_winners(lane, W, P, g, 0, 1, false));                          \
     }                                                                                  \
     if (bc7_full_two(P)) {                                                             \
