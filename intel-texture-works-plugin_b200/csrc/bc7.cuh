@@ -1,9 +1,10 @@
 // bc7.cuh -- BC7 encoder (reference: kernel.ispc:616-2037, cited as K:line).
 //
-// Mapping.  One WARP owns kBc7Super = 16 consecutive 4x4 blocks per round (kBc7Batch = 8 on surfaces too small to give
-// every SM such a CTA).  The shape / ranking phases hold one HALF of eight blocks at a time, as two GROUPS of kBc7Slots = 4
-// that reuse the per-group scratch; the chain phase -- 14 to 18 roles per block, a quarter of the work -- runs ONCE for all
-// sixteen blocks, two lanes per block, so that a pass is two equally long roles wide (DESIGN.md section 4 has the numbers).
+// Mapping.  One WARP owns kBc7Super = 16 consecutive 4x4 blocks per full round (the last round of a launch deals what is left
+// over every warp of the grid, 1 to 16 blocks each; bc7_kernel).  The shape / ranking phases hold one HALF of eight blocks at
+// a time, as two GROUPS of kBc7Slots = 4 that reuse the per-group scratch; the chain phase -- 14 to 18 roles per block, a
+// quarter of the work -- runs ONCE for all sixteen blocks, two lanes per block, so that a pass is two equally long roles wide
+// (DESIGN.md section 4 has the numbers).
 // The 32 lanes are spread over the blocks' independent work items instead of over texels:
 //   * shape phases: a shape's error is the sum of its subsets' errors, and a subset's fit, endpoints and error depend on its
 //     texel mask alone (the reference refits per shape and mode, K:1279-1297, with identical results).  So the three-subset
@@ -17,7 +18,9 @@
 //     texels scores modes 1 and 3.  For shorter lists and for mode 7 a lane evaluates one ranked shape: it fits each subset
 //     and searches the shape for both modes of the pair (the pair fit measured slower there: it raises the register
 //     pressure of bc7_eval_shape);
-//   * ranking phase: lane <-> (block slot, two-subset shape) for the 64 PCA split bounds;
+//   * ranking phase: lane <-> (block slot, two-subset shape) for the 64 PCA split bounds, only where a list of 0 < t < 64
+//     shapes needs it to choose its members;
+//   * winner phases: lane <-> (block slot, list, strip of 16 entries), then lane <-> (block slot, list);
 //   * chain phase: lane <-> (block slot, role).  The per-mode refinement chains, the mode 4/5
 //     rotation / index-swap candidates and mode 6 are independent of one another in the reference
 //     (they only meet in a strict `<` on the final error, K:1358, :1638, :1650, :1684), so they
@@ -71,8 +74,9 @@ struct Bc7Params {
 
 constexpr int kBc7Slots = 4;          // blocks per group (ranking / shape phases share per-group scratch)
 constexpr int kBc7Batch = 8;          // blocks per HALF: what the shape phases hold in Bc7Warp::blk at a time (two groups)
-constexpr int kBc7Super = 16;         // blocks per warp and round when the surface is large: two halves, ONE chain phase
+constexpr int kBc7Super = 16;         // blocks per warp in a full round: two halves, ONE chain phase
 constexpr int kBc7MaxRoles = 18;      // 5 partitioned modes + up to 8 mode-4 + 4 mode-5 + mode 6
+constexpr int kBc7Strips = 4;         // a candidate list of up to 64 entries is reduced in four strips of 16
 constexpr int kErrNone = 0x7fffffff;  // "no result": loses every strict < comparison
 
 // One 4x4 block in shared memory
@@ -98,8 +102,14 @@ struct Bc7Warp {
     };
     uint8_t order[kBc7Slots][2][64];           // shapes in ascending key order: [0] RGB (modes 1,3), [1] profile channels (mode 7)
     int win_shape[kBc7Super][5];               // winning shape id per block of the round and mode slot, -1 = none
-    u32 palette[40][32];                       // lane-private scratch of the index search, [entry][lane]: 24 palette
+    union {
+        u32 palette[40][32];                   // lane-private scratch of the index search, [entry][lane]: 24 palette
                                                // entries, then 5 per-subset constants x 3 subsets
+        // winner selection (no index search runs then): the best (error, list position) of each strip of 16 list entries
+        struct {
+            int err[kBc7Strips][kBc7Slots][2], pos[kBc7Strips][kBc7Slots][2];
+        } strip;
+    };
     union {
         // every DISTINCT three-subset mask, for the four blocks of the group (bc7_phase_masks3 -> bc7_phase_shapes3): the
         // mode-2 subset error of all 140 masks, the decoded mode-0 endpoints (A, B as RGBA bytes) of the 36 masks of shapes 0..15
@@ -133,11 +143,15 @@ ITW_HD int bc7_slot_count(const Bc7Params& P, int m)
     if (m == 3) return P.sel[1] ? P.t3 : 0;
     return P.sel[1] ? P.t7 : 0;
 }
+// A two-subset list that holds all 64 shapes is walked in shape order and never ranked: its winner, the first minimum in
+// ranked (ascending key) order, is the minimum of (error, key), since the keys are unique (bc7_phase_strips).
+ITW_HD bool bc7_shape_order(const Bc7Params& P, int m) { return m >= 2 && bc7_slot_count(P, m) == 64; }
 // shape id of list position n of mode slot m
-ITW_HD int bc7_slot_shape(const Bc7Warp& W, int slot, int m, int n)
+ITW_HD int bc7_slot_shape(const Bc7Warp& W, const Bc7Params& P, int slot, int m, int n)
 {
     if (m <= 1) return 64 + n;                                  // modes 0/2 walk the 3-subset table in order
-    return W.order[slot][(m == 4) ? 1 : 0][n] & 63;             // modes 1/3/7 walk the ranked list
+    if (bc7_shape_order(P, m)) return n;
+    return W.order[slot][(m == 4) ? 1 : 0][n] & 63;             // shorter lists of modes 1/3/7 walk the ranked list
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1401,7 +1415,7 @@ ITW_HD void bc7_phase_shapes(int lane, Bc7Warp& W, const Bc7Params& P, int g, in
         int slot, n;
         if (t < nboth) { slot = t / both; n = t - slot * both; }
         else { const int u = t - nboth, rest = count - both; slot = u / rest; n = both + (u - slot * rest); }
-        bc7_eval_shape(W, lane, slot, &W.blk[kBc7Slots * g + slot], bc7_slot_shape(W, slot, ma, n), n, ma, n < ca, mb, n < cb);
+        bc7_eval_shape(W, lane, slot, &W.blk[kBc7Slots * g + slot], bc7_slot_shape(W, P, slot, ma, n), n, ma, n < ca, mb, n < cb);
     }
 }
 // split-bound keys of the 64 two-subset shapes; set 0 = RGB (modes 1,3), set 1 = profile channels (mode 7)
@@ -1451,6 +1465,13 @@ ITW_HD void bc7_phase_two_full(int lane, Bc7Warp& W, const Bc7Params& P, int g)
         W.two.keys[slot][shape] = bc7_key_of(shape, f.bound[0], f.bound[1]);
     }
 }
+// The ranking decides which shapes a list of 0 < t < 64 entries holds; a list of all 64 is walked in shape order instead.
+ITW_HD bool bc7_needs_rank(const Bc7Params& P, int set)
+{
+    for (int m = set ? 4 : 2; m <= (set ? 4 : 3); m++)
+        if (bc7_slot_count(P, m) > 0 && bc7_slot_count(P, m) < 64) return true;
+    return false;
+}
 ITW_HD void bc7_phase_rank(int lane, Bc7Warp& W, int g, int set)
 {
     for (int t = lane; t < bc7_group_count(W, g) * 64; t += 32) {
@@ -1458,9 +1479,64 @@ ITW_HD void bc7_phase_rank(int lane, Bc7Warp& W, int g, int set)
         W.order[slot][set][rank_of(W.two.keys[slot], 64, i)] = (uint8_t)(W.two.keys[slot][i] & 63);
     }
 }
-// first minimum of the candidate lists just evaluated for mode slots (ma, mb) of group g, as a SHAPE id; K:1320 (strict <).
-// by_shape: the errors are stored by shape id, not by list position (bc7_phase_two_full).
-ITW_HD void bc7_phase_winners(int lane, Bc7Warp& W, const Bc7Params& P, int g, int ma, int mb, bool by_shape)
+// Winners of lists that hold all 64 two-subset shapes (and of a short list evaluated next to such a list), for mode slots
+// (ma, mb) of group g: the first minimum in list order; K:1320
+// (strict <, so an error of kErrNone never wins and an empty list gives -1).  That is the minimum of (error, tie), where the tie
+// is the list position, or the ranking key for a list in shape order (bc7_shape_order; keys compare as signed ints, as in
+// rank_of).  by_shape: the errors are stored by shape id, not by list position (bc7_phase_two_full).
+// Two phases: bc7_phase_strips, lane <-> (block, list, strip of 16 entries), then bc7_phase_winners, lane <-> (block, list),
+// which combines the four strips.  The strip routine is not inlined (inlined into the kernel, it made bc7_chain spill 72 bytes
+// instead of 4, -Xptxas -v) and takes the list lengths by value (a Bc7Params by reference would be read from local memory).
+ITW_HD_NOINLINE void bc7_strips(int lane, Bc7Warp& W, int g, int nm, int ca, int cb, bool two, bool by_shape)
+{
+    for (int t = lane; t < bc7_group_count(W, g) * nm * kBc7Strips; t += 32) {
+        const int strip = t % kBc7Strips, list = t / kBc7Strips, slot = list / nm, which = list - slot * nm;
+        const int count = which ? cb : ca;
+        const bool keyed = two && count == 64;                        // bc7_shape_order
+        const bool ranked = by_shape && !keyed;                       // errors by shape id, entries in ranked order
+        const int* err = W.cand_err[slot][which];
+        int best = -1, best_err = kErrNone, best_tie = 0;
+        // the lanes of a strip parity start at 16 different entries: entry n of (slot, which, strip) lies in bank
+        // (16 strip + n) % 32 of cand_err and of the keys, so reading the strips in step was a 16-way bank conflict.  The
+        // comparison is on (error, tie), so the order of the walk does not matter.
+        const int rot = (t >> 1) & 15;
+#pragma unroll 1
+        for (int i = 0; i < 16; i++) {
+            const int n = 16 * strip + ((i + rot) & 15);
+            if (n < count) {
+                const int e = err[ranked ? (W.order[slot][0][n] & 63) : n];
+                const int tie = keyed ? W.two.keys[slot][n] : n;
+                if (e < best_err || (e == best_err && best >= 0 && tie < best_tie)) { best_err = e; best = n; best_tie = tie; }
+            }
+        }
+        W.strip.err[strip][slot][which] = best_err;
+        W.strip.pos[strip][slot][which] = best;
+    }
+}
+ITW_HD void bc7_phase_strips(int lane, Bc7Warp& W, const Bc7Params& P, int g, int ma, int mb, bool by_shape)
+{
+    bc7_strips(lane, W, g, (mb != ma) ? 2 : 1, bc7_slot_count(P, ma), (mb != ma) ? bc7_slot_count(P, mb) : 0, ma >= 2, by_shape);
+}
+ITW_HD void bc7_phase_winners(int lane, Bc7Warp& W, const Bc7Params& P, int g, int ma, int mb)
+{
+    const int nm = (mb != ma) ? 2 : 1;
+    for (int t = lane; t < bc7_group_count(W, g) * nm; t += 32) {
+        const int slot = t / nm, which = t - slot * nm;
+        const int m = which ? mb : ma;
+        const bool keyed = bc7_shape_order(P, m);
+        int best = -1, best_err = kErrNone, best_tie = 0;
+        for (int s = 0; s < kBc7Strips; s++) {
+            const int e = W.strip.err[s][slot][which], n = W.strip.pos[s][slot][which];
+            if (n < 0) continue;
+            const int tie = keyed ? W.two.keys[slot][n] : n;
+            if (e < best_err || (e == best_err && best >= 0 && tie < best_tie)) { best_err = e; best = n; best_tie = tie; }
+        }
+        W.win_shape[kBc7Batch * W.half + kBc7Slots * g + slot][m] = (best < 0) ? -1 : bc7_slot_shape(W, P, slot, m, best);
+    }
+}
+// Lists in list order (modes 0 / 2, ranked lists) keep one phase: lane <-> (block, list) walks the list.  Through the strip
+// phases they measured slower on basic (+0.5 %, H100): their lists are at most 16 entries long except mode 2's.
+ITW_HD void bc7_phase_first_min(int lane, Bc7Warp& W, const Bc7Params& P, int g, int ma, int mb)
 {
     const int nm = (mb != ma) ? 2 : 1;
     for (int t = lane; t < bc7_group_count(W, g) * nm; t += 32) {
@@ -1469,23 +1545,23 @@ ITW_HD void bc7_phase_winners(int lane, Bc7Warp& W, const Bc7Params& P, int g, i
         const int count = bc7_slot_count(P, m);
         int best = -1, best_err = kErrNone;
         for (int n = 0; n < count; n++) {
-            const int e = W.cand_err[slot][which][by_shape ? bc7_slot_shape(W, slot, m, n) : n];
+            const int e = W.cand_err[slot][which][n];
             if (e < best_err) { best_err = e; best = n; }
         }
-        W.win_shape[kBc7Batch * W.half + kBc7Slots * g + slot][m] = (best < 0) ? -1 : bc7_slot_shape(W, slot, m, best);
+        W.win_shape[kBc7Batch * W.half + kBc7Slots * g + slot][m] = (best < 0) ? -1 : bc7_slot_shape(W, P, slot, m, best);
     }
 }
-// Chain phase over the whole round.  With nb = 16 (two halves) or 8 blocks, lane L works for block L % nb in every pass and
-// runs the active roles L / nb, L / nb + 32 / nb, ...: a pass holds 32 / nb consecutive roles for all blocks, so its lanes run
-// the same KIND of role (partitioned / mode 4-5 / mode 6) almost everywhere, and a lane keeps the best candidate of ITS block
-// in registers.  Sixteen blocks make a pass two roles wide: (mode 0, mode 2), (mode 1, mode 3), (rotation, rotation), ... are
-// equally long, where four-wide passes pair three-subset with two-subset chains and leave the last pass half empty.
+// Chain phase over the whole round.  With nb = per_warp blocks (a power of two, 1..16), lane L works for block L % nb in every
+// pass and runs the active roles L / nb, L / nb + 32 / nb, ...: a pass holds 32 / nb consecutive roles for all blocks, so its
+// lanes run the same KIND of role (partitioned / mode 4-5 / mode 6) almost everywhere, and a lane keeps the best candidate of
+// ITS block in registers.  Sixteen blocks make a pass two roles wide: (mode 0, mode 2), (mode 1, mode 3), (rotation, rotation),
+// ... are equally long, where four-wide passes pair three-subset with two-subset chains and leave the last pass half empty.
+// Fewer blocks (the last round of a launch) run wider passes: with one block, all its roles run in one pass.
 // The first strict minimum in role order is kept (K:1358, :1638, :1650, :1684): a lane meets its roles in ascending order,
 // the store phase compares (error, role).
-ITW_HD void bc7_phase_chains(int lane, Bc7Warp& W, const Bc7Params& P)
+ITW_HD void bc7_phase_chains(int lane, Bc7Warp& W, const Bc7Params& P, int nb)
 {
     const int nactive = bc7_active_roles(P);
-    const int nb = (W.ntotal > kBc7Batch) ? kBc7Super : kBc7Batch;
     const int slot = lane & (nb - 1);
     int best_err = kErrNone, best_role = 0;
     u32 code[4] = {0u, 0u, 0u, 0u};
@@ -1505,10 +1581,8 @@ ITW_HD void bc7_phase_chains(int lane, Bc7Warp& W, const Bc7Params& P)
     for (int i = 0; i < 4; i++) W.fin.code[lane][i] = code[i];
 }
 // the block's winner among the lanes that worked for it, then the 16-byte store; K:2027
-ITW_HD void bc7_phase_store(int lane, Bc7Warp& W, const Bc7Params& P, uint8_t* dst, long long first_block)
+ITW_HD void bc7_phase_store(int lane, Bc7Warp& W, int nb, uint8_t* dst, long long first_block)
 {
-    (void)P;
-    const int nb = (W.ntotal > kBc7Batch) ? kBc7Super : kBc7Batch;
     for (int t = lane; t < W.ntotal; t += 32) {
         int best = t;
         for (int j = 1; j < 32 / nb; j++) {
@@ -1521,39 +1595,49 @@ ITW_HD void bc7_phase_store(int lane, Bc7Warp& W, const Bc7Params& P, uint8_t* d
     }
 }
 
-// The program of one round (up to kBc7Super blocks: `nvalid` of them from `first_block` of `surf`, results to block
-// `out_block` of `dst`), as a list of (phase, barrier) pairs.
+// The program of one round (per_warp = 1, 2, 4, 8 or 16 blocks per warp: `nvalid` of them from `first_block` of `surf`,
+// results to block `out_block` of `dst`), as a list of (phase, barrier) pairs.
 #define ITW_BC7_GROUP_PROGRAM(PHASE, g)                                                \
     if (P.sel[0]) {                                                                    \
         PHASE(bc7_phase_masks3(lane, W, P, g));                                        \
         PHASE(bc7_phase_shapes3(lane, W, P, g));                                       \
-        PHASE(bc7_phase_winners(lane, W, P, g, 0, 1, false));                          \
+        PHASE(bc7_phase_first_min(lane, W, P, g, 0, 1));                               \
     }                                                                                  \
     if (bc7_full_two(P)) {                                                             \
         PHASE(bc7_phase_two_full(lane, W, P, g));                                      \
-        PHASE(bc7_phase_rank(lane, W, g, 0));                                          \
-        PHASE(bc7_phase_winners(lane, W, P, g, 2, 3, true));                           \
+        if (bc7_needs_rank(P, 0)) {                                                    \
+            PHASE(bc7_phase_rank(lane, W, g, 0));                                      \
+        }                                                                              \
+        PHASE(bc7_phase_strips(lane, W, P, g, 2, 3, true));                            \
+        PHASE(bc7_phase_winners(lane, W, P, g, 2, 3));                                 \
     } else if (bc7_needs_keys(P, 0)) {                                                 \
         PHASE(bc7_phase_keys(lane, W, P, g, 0));                                       \
         PHASE(bc7_phase_rank(lane, W, g, 0));                                          \
         PHASE(bc7_phase_shapes(lane, W, P, g, 2, 3));                                  \
-        PHASE(bc7_phase_winners(lane, W, P, g, 2, 3, false));                          \
+        PHASE(bc7_phase_first_min(lane, W, P, g, 2, 3));                               \
     }                                                                                  \
     if (bc7_needs_keys(P, 1)) {                                                        \
         PHASE(bc7_phase_keys(lane, W, P, g, 1));                                       \
-        PHASE(bc7_phase_rank(lane, W, g, 1));                                          \
-        PHASE(bc7_phase_shapes(lane, W, P, g, 4, 4));                                  \
-        PHASE(bc7_phase_winners(lane, W, P, g, 4, 4, false));                          \
+        if (bc7_needs_rank(P, 1)) {                                                    \
+            PHASE(bc7_phase_rank(lane, W, g, 1));                                      \
+            PHASE(bc7_phase_shapes(lane, W, P, g, 4, 4));                              \
+            PHASE(bc7_phase_first_min(lane, W, P, g, 4, 4));                           \
+        } else {                                                                       \
+            PHASE(bc7_phase_shapes(lane, W, P, g, 4, 4));                              \
+            PHASE(bc7_phase_strips(lane, W, P, g, 4, 4, false));                       \
+            PHASE(bc7_phase_winners(lane, W, P, g, 4, 4));                             \
+        }                                                                              \
     }
 // The halves and the groups are LOOPS, not copies: four inlined copies of every shape phase made the kernel body 6.6 k
-// instructions (105 KB) -- the phases of one copy are what the instruction cache should hold.
+// instructions (105 KB) -- the phases of one copy are what the instruction cache should hold.  A round of at most four blocks
+// per warp has one group.
 #define ITW_BC7_SHAPE_PROGRAM(PHASE)                                                   \
     ITW_UNROLL(1)                                                                      \
     for (int half = 0; half < ((per_warp > kBc7Batch) ? 2 : 1); half++) {              \
         PHASE(bc7_phase_load(lane, W, surf, first_block, nvalid, half));               \
         PHASE(bc7_phase_planes(lane, W));                                              \
         ITW_UNROLL(1)                                                                  \
-        for (int g = 0; g < kBc7Batch / kBc7Slots; g++) {                              \
+        for (int g = 0; g < ((per_warp > kBc7Slots) ? 2 : 1); g++) {                   \
             ITW_BC7_GROUP_PROGRAM(PHASE, g)                                            \
         }                                                                              \
     }                                                                                  \
@@ -1561,8 +1645,8 @@ ITW_HD void bc7_phase_store(int lane, Bc7Warp& W, const Bc7Params& P, uint8_t* d
         PHASE(bc7_phase_park(lane, W, surf, first_block, nvalid));                     \
     }
 #define ITW_BC7_CHAIN_PROGRAM(PHASE)                                                   \
-    PHASE(bc7_phase_chains(lane, W, P));                                               \
-    PHASE(bc7_phase_store(lane, W, P, dst, out_block));
+    PHASE(bc7_phase_chains(lane, W, P, per_warp));                                     \
+    PHASE(bc7_phase_store(lane, W, per_warp, dst, out_block));
 #define ITW_BC7_PROGRAM(PHASE)                                                         \
     ITW_BC7_SHAPE_PROGRAM(PHASE)                                                       \
     ITW_BC7_CHAIN_PROGRAM(PHASE)
@@ -1581,56 +1665,116 @@ constexpr size_t kBc7SmemBytes = sizeof(Bc7Warp) * kBc7WarpsPerCta;
 // from shared memory.  One tile buffer is enough: it is free again once the last load phase of a round is over, and the next
 // tile then streams in behind the whole chain phase.  Needs 16-byte aligned surface rows; other surfaces use the plain
 // global-load variant.
-// per_warp = kBc7Super for surfaces large enough to give every warp of the grid 16 blocks, kBc7Batch for small ones (more warps
-// busy; the chain phase then runs four roles wide).
 constexpr int kBc7TileBlocks = kBc7WarpsPerCta * kBc7Super;              // 256
 constexpr int kBc7TileRowBytes = kBc7TileBlocks * 16;                     // 4096
 
+#if defined(ITW_BC7_PHASE_CLOCKS)
+// Per-phase cycle attribution (tools/bc7_phase_clocks.py; not in the product build): thread 0 of every CTA reads clock64()
+// after every barrier and adds the cycles since its previous reading to the phase site it just left.  Sites are numbered in
+// the order the program macros expand them.
+constexpr int kBc7ClockSites = 40;
+struct Bc7Clocks {
+    unsigned long long site[kBc7ClockSites];     // cycles summed over the CTAs
+    char name[kBc7ClockSites][48];               // the phase call of each site
+    unsigned long long full_sum, full_count;     // cycles of the full rounds (summed) and their number, over the CTAs
+    unsigned long long last_sum, last_max, last_ctas;   // the partial last round: summed, longest CTA, CTAs that ran it
+};
+__device__ Bc7Clocks g_bc7_clocks;
+__device__ void bc7_clock_tick(int site, const char* name, unsigned long long& last)
+{
+    const unsigned long long now = clock64();
+    atomicAdd(&g_bc7_clocks.site[site], now - last);
+    last = now;
+    if (blockIdx.x == 0 && g_bc7_clocks.name[site][0] == 0)
+        for (int i = 0; i < 47 && name[i]; i++) g_bc7_clocks.name[site][i] = name[i];
+}
+#define ITW_BC7_TICK(name) if (threadIdx.x == 0) bc7_clock_tick(__COUNTER__ - clock_site0, name, clock_last)
+#else
+#define ITW_BC7_TICK(name)
+#endif
+
+// Schedule.  A full round gives every warp of the grid kBc7Super blocks: wave = grid x 16 warps x 16 blocks.  The blocks left
+// after the full rounds (fewer than a wave) are dealt over ALL warps of the grid as one last round of per_warp = 1, 2, 4, 8 or
+// 16 blocks, the smallest that covers them, instead of a sixteen-block round of the first few CTAs while the other SMs idle.
+// Warps stay CTA-major, so a CTA's share of a round is one contiguous run of blocks (one TMA tile).  Small surfaces are the
+// same case with zero full rounds.
 template <bool kTma>
 __global__ void __launch_bounds__(kBc7WarpsPerCta * 32, 1)
-bc7_kernel(SurfaceView gsurf, uint8_t* __restrict__ dst, Bc7Params P, long long nblocks, int per_warp)
+bc7_kernel(SurfaceView gsurf, uint8_t* __restrict__ dst, Bc7Params P, long long nblocks)
 {
     extern __shared__ __align__(16) unsigned char bc7_smem[];
     __shared__ __align__(128) unsigned char stage[kTma ? 4 * kBc7TileRowBytes : 16];
     __shared__ __align__(8) unsigned long long full;
     Bc7Warp& W = reinterpret_cast<Bc7Warp*>(bc7_smem)[threadIdx.x >> 5];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const long long nbatches = (nblocks + per_warp - 1) / per_warp;
-    const long long nwarps = (long long)gridDim.x * kBc7WarpsPerCta;
-    const long long rounds = (nbatches + nwarps - 1) / nwarps;            // same trip count for every warp of the CTA
-    const int tile_blocks = kBc7WarpsPerCta * per_warp;
-
-    auto tile_first = [&](long long round) { return ((long long)blockIdx.x * kBc7WarpsPerCta + round * nwarps) * per_warp; };
-    auto prefetch = [&](long long round) {                                // one thread feeds the TMA engine
-        const long long fb = tile_first(round);
-        if (round >= rounds || fb >= nblocks) return;
+    // The schedule lives in shared memory and is read again in every round: held in registers across the phases, it added 40
+    // bytes to the kernel's spills at the 128-register cap (-Xptxas -v).  Round counters are ints (a round is at least 16 blocks).
+    __shared__ int sched[2];                                              // full rounds; blocks per warp of the last one (0: none)
+    if (threadIdx.x == 0) {
+        const long long wave = (long long)gridDim.x * kBc7TileBlocks;
+        const long long nfull = nblocks / wave, rem = nblocks - nfull * wave;
+        int p = 0;
+        if (rem > 0)
+            for (p = 1; p < kBc7Super && (rem + p - 1) / p > (long long)gridDim.x * kBc7WarpsPerCta; p *= 2) {}
+        sched[0] = (int)nfull;
+        sched[1] = p;
+    }
+    auto round_per_warp = [&](int round) { return round < sched[0] ? kBc7Super : (round == sched[0] ? sched[1] : 0); };
+    auto tile_first = [&](int round) {
+        return round * ((long long)gridDim.x * kBc7TileBlocks) + (long long)blockIdx.x * kBc7WarpsPerCta * round_per_warp(round);
+    };
+    auto prefetch = [&](int round) {                                      // one thread feeds the TMA engine
+        const long long fb = tile_first(round), tile_blocks = (long long)kBc7WarpsPerCta * round_per_warp(round);
+        if (tile_blocks == 0 || fb >= nblocks) return;
         const long long left = nblocks - fb;
         tma_prefetch_tile(stage, kBc7TileRowBytes, &full, gsurf, fb, (int)(left < tile_blocks ? left : tile_blocks), 16);
     };
-    if (kTma) {
-        if (threadIdx.x == 0) mbar_init(&full, 1);
-        __syncthreads();
-        if (threadIdx.x == 0) prefetch(0);
-    }
-    for (long long round = 0; round < rounds; round++) {
-        const long long batch = (long long)blockIdx.x * kBc7WarpsPerCta + warp + round * nwarps;
-        const long long out_block = batch * per_warp;
+#if defined(ITW_BC7_PHASE_CLOCKS)
+    const int clock_site0 = __COUNTER__;
+    unsigned long long clock_last = clock64();
+#endif
+    if (kTma && threadIdx.x == 0) mbar_init(&full, 1);
+    __syncthreads();
+    if (kTma && threadIdx.x == 0) prefetch(0);
+    for (int round = 0;; round++) {
+        const int per_warp = round_per_warp(round);
+        const long long cta_first = tile_first(round);
+        if (per_warp == 0 || cta_first >= nblocks) break;               // all done, or nothing for this CTA in the last round
+#if defined(ITW_BC7_PHASE_CLOCKS)
+        const unsigned long long round_start = clock_last;
+#endif
+        const long long out_block = cta_first + (long long)warp * per_warp;
         const long long left = nblocks - out_block;
         const int nvalid = (int)(left <= 0 ? 0 : (left < per_warp ? left : per_warp));
         SurfaceView surf = gsurf;
         long long first_block = out_block;
         if (kTma) {
-            if (tile_first(round) < nblocks) mbar_wait(&full, (unsigned)(round & 1));
+            mbar_wait(&full, (unsigned)(round & 1));
             surf = SurfaceView{stage, kBc7TileBlocks * 4, 4, kBc7TileRowBytes};
             first_block = (long long)warp * per_warp;                    // block index inside the staged tile
         }
-#define ITW_PHASE_DEVICE(call) call; __syncthreads()
+        ITW_BC7_TICK("round start (TMA wait)");
+#define ITW_PHASE_DEVICE(call) call; __syncthreads(); ITW_BC7_TICK(#call)
         ITW_BC7_SHAPE_PROGRAM(ITW_PHASE_DEVICE)
         if (kTma && threadIdx.x == 0) prefetch(round + 1);               // every load phase of this round is behind a barrier
         ITW_BC7_CHAIN_PROGRAM(ITW_PHASE_DEVICE)
 #undef ITW_PHASE_DEVICE
+#if defined(ITW_BC7_PHASE_CLOCKS)
+        if (threadIdx.x == 0) {
+            const unsigned long long cycles = clock_last - round_start;
+            if (per_warp == kBc7Super && round < sched[0]) {
+                atomicAdd(&g_bc7_clocks.full_sum, cycles);
+                atomicAdd(&g_bc7_clocks.full_count, 1ull);
+            } else {
+                atomicAdd(&g_bc7_clocks.last_sum, cycles);
+                atomicMax(&g_bc7_clocks.last_max, cycles);
+                atomicAdd(&g_bc7_clocks.last_ctas, 1ull);
+            }
+        }
+#endif
     }
 }
+#undef ITW_BC7_TICK
 #endif
 
 }  // namespace itw

@@ -239,16 +239,15 @@ int launch(const Encoder& e, const SurfaceView& v, uint8_t* d_dst, cudaStream_t 
             else       bc4_bc5_kernel<true, false><<<grid1, 128, 0, stream>>>(v, d_dst);
             break;
         case ITW_FORMAT_BC7: {
-            // one 16-warp CTA per SM, persistent over the rounds; TMA-staged variant when the surface allows it.  A warp takes 16
-            // blocks per round when that still gives every SM a full CTA, else 8 (small surfaces / row bands: more warps busy)
+            // one 16-warp CTA per SM, persistent over the rounds; TMA-staged variant when the surface allows it.  The kernel
+            // owns the schedule (how many blocks a warp takes per round); a surface of fewer than SMs x 16 blocks gets one CTA
+            // per 16 blocks
             const bool tma = vec16;                                       // 16-byte aligned rows
             const long long cap = (long long)tls.sm_count;
-            const int per_warp = (nblocks >= cap * kBc7WarpsPerCta * kBc7Super) ? kBc7Super : kBc7Batch;
-            const long long tile = (long long)kBc7WarpsPerCta * per_warp;
-            const long long want = (nblocks + tile - 1) / tile;
+            const long long want = (nblocks + kBc7WarpsPerCta - 1) / kBc7WarpsPerCta;
             const unsigned grid = (unsigned)(want < cap ? want : cap);
-            if (tma) bc7_kernel<true><<<grid, kBc7WarpsPerCta * 32, kBc7SmemBytes, stream>>>(v, d_dst, e.bc7, nblocks, per_warp);
-            else     bc7_kernel<false><<<grid, kBc7WarpsPerCta * 32, kBc7SmemBytes, stream>>>(v, d_dst, e.bc7, nblocks, per_warp);
+            if (tma) bc7_kernel<true><<<grid, kBc7WarpsPerCta * 32, kBc7SmemBytes, stream>>>(v, d_dst, e.bc7, nblocks);
+            else     bc7_kernel<false><<<grid, kBc7WarpsPerCta * 32, kBc7SmemBytes, stream>>>(v, d_dst, e.bc7, nblocks);
             break;
         }
         case ITW_FORMAT_BC6H: {
@@ -1018,6 +1017,20 @@ float itw_last_kernel_ms(void)
     if (tls.timed && cudaEventElapsedTime(&ms, tls.ev0, tls.ev1) != cudaSuccess) { cudaGetLastError(); ms = -1.0f; }
     return ms;
 }
+
+#if defined(ITW_BC7_PHASE_CLOCKS)
+// Measurement build only (tools/bc7_phase_clocks.py): copies the per-phase cycle counters of bc7_kernel (a Bc7Clocks, `bytes`
+// must be its size) to `out` after the work enqueued so far has finished, then zeroes them.
+int itw_bc7_phase_clocks(void* out, size_t bytes)
+{
+    if (bytes != sizeof(Bc7Clocks)) return fail("itw_bc7_phase_clocks: wrong size");
+    ITW_CUDA(cudaDeviceSynchronize());
+    ITW_CUDA(cudaMemcpyFromSymbol(out, g_bc7_clocks, sizeof(Bc7Clocks)));
+    static const Bc7Clocks zero{};
+    ITW_CUDA(cudaMemcpyToSymbol(g_bc7_clocks, &zero, sizeof(Bc7Clocks)));
+    return 0;
+}
+#endif
 
 }  // extern "C"
 
