@@ -9,12 +9,12 @@
 //   * shape phases: a shape's error is the sum of its subsets' errors, and a subset's fit, endpoints and error depend on its
 //     texel mask alone (the reference refits per shape and mode, K:1279-1297, with identical results).  So the three-subset
 //     shapes go lane <-> (block, two distinct masks) over the four blocks of a group: one routine fits both masks
-//     (bc7_fit_masks2: two moment passes, two independent power iterations, one projection loop), quantises them for modes 0
+//     (bc7_fit_masks2: two moment passes, two independent PCA lines, one projection loop), quantises them for modes 0
 //     and 2, and one walk over both masks' texels searches them for mode 2; then lane <-> (block, shape) adds three stored
 //     mode-2 errors and searches mode 0 from the stored endpoints.  A two-subset shape
 //     (modes 1, 3, 7) belongs to one lane.  When the profile searches all 64 of them for modes 1 / 3, lane <-> (block, shape)
 //     over the four blocks of a group: one routine fits both subsets (bc7_fit_pair: subset 1's moments are the block's minus
-//     subset 0's, two independent power iterations, one projection loop) and gives the split keys, and one walk over the 16
+//     subset 0's, two independent PCA lines, one projection loop) and gives the split keys, and one walk over the 16
 //     texels scores modes 1 and 3.  For shorter lists and for mode 7 a lane evaluates one ranked shape: it fits each subset
 //     and searches the shape for both modes of the pair (the pair fit measured slower there: it raises the register
 //     pressure of bc7_eval_shape);
@@ -38,7 +38,9 @@
 //     them through int, K:1172-1173) and their squared errors are VABSDIFF4 + IDP.4A;
 //   * least-squares sums (K:1198-1230): IDP.4A over index bytes.
 // Everything that rounds (covariance, power iteration, endpoint solve, quantisation) follows the
-// reference's float expression order exactly (DESIGN.md "Canonical float model").
+// reference's float expression order exactly (DESIGN.md "Canonical float model").  Every fit goes through one PCA-line
+// routine (bc7_line, bc7_project, bc7_ends) and every index search through one texel step (bc7_num, bc7_q1_quotient /
+// bc7_steps, bc7_pick), so the variants cannot round differently.
 //
 // Structure for speed (DESIGN.md section 4): the non-inlined routines exchange their results BY VALUE (small structs stay
 // in registers across calls; arrays passed by pointer would live in local memory), the inner routines are branch-free
@@ -311,72 +313,98 @@ ITW_HD float bc7_bound_from_axis(const float (&cov)[10], const float (&axis)[4])
     bound -= sqrtf(sum);
     return max_sse(bound, 0.0f);
 }
-// kBound: also the split bound of the mask (bc7_residual_bound).  At three channels the fit's scaled covariance equals the
-// bound's (the eps the fit adds to slot 9 is never read), and the bound's four power iterations are the fit's first four.
-template <int CH, bool kBound>
-ITW_HD void bc7_fit_impl(float (&ep)[8], float& bound, const View& v, u32 mask)
+// Scales a covariance by 1/256^2 and adds eps to its diagonal.  The fit puts eps on all four diagonal slots (K:842-852); the
+// split bound on three only (K:911-920), so a four-channel bound differs from the fit's in slot 9.
+template <bool kEps9>
+ITW_HD void bc7_scale_covariance(float (&cov)[10])
 {
-    static_assert(!kBound || CH == 3, "the four-channel fit adds eps to slot 9, the split bound does not");
-    u32 P[4][4];
-    load_planes(P, v);
-    int ist[15];
-    moments_u8(ist, P, mask, CH);
-    float cov[10], mean[4];
-    bc7_covariance<CH>(cov, mean, ist);
     const float inv_var = 1.0f / (256.0f * 256.0f);
 #pragma unroll
     for (int i = 0; i < 10; i++) cov[i] *= inv_var;
     const float eps = 0.001f * 0.001f;
-    cov[0] += eps; cov[4] += eps; cov[7] += eps; cov[9] += eps;
-    float axis[4] = {1.0f, 1.0f, 1.0f, 1.0f};
-    bc7_power_axis<CH, 4>(axis, cov);
-    if (kBound) bound = bc7_bound_from_axis<CH>(cov, axis);
-    bc7_power_axis<CH, 4>(axis, cov);
-
+    cov[0] += eps; cov[4] += eps; cov[7] += eps;
+    if (kEps9) cov[9] += eps;
+}
+// The PCA line of a set of moments (K:834-855): mean and principal axis after eight power iterations.  kBound: also the split
+// bound of the mask (bc7_residual_bound).  At three channels the fit's scaled covariance equals the bound's (slot 9 is never
+// read), and the bound's four power iterations are the fit's first four.
+struct Bc7Line { float axis[4], mean[4], bound; };
+template <int CH, bool kBound>
+ITW_HD Bc7Line bc7_line(const int (&st)[15])
+{
+    static_assert(!kBound || CH == 3, "the four-channel fit adds eps to slot 9, the split bound does not");
+    Bc7Line l;
+    float cov[10];
+    bc7_covariance<CH>(cov, l.mean, st);
+    bc7_scale_covariance<true>(cov);
+#pragma unroll
+    for (int c = 0; c < 4; c++) l.axis[c] = 1.0f;
+    bc7_power_axis<CH, 4>(l.axis, cov);
+    l.bound = kBound ? bc7_bound_from_axis<CH>(cov, l.axis) : 0.0f;
+    bc7_power_axis<CH, 4>(l.axis, cov);
+    return l;
+}
+// Position of texel k along a line through `mean` (K:874-876).  The reference starts the sum from 0.0f; 0 + x differs from
+// x only in the sign of a zero, which nothing downstream can observe (bc7_fit), so the sum starts from the first product.
+template <int CH>
+ITW_HD float bc7_project(const float (&axis)[4], const float (&mean)[4], const u32 (&P)[4][4], int k)
+{
+    float d = axis[0] * ((float)((P[0][k >> 2] >> (8 * (k & 3))) & 255u) - mean[0]);
+#pragma unroll
+    for (int c = 1; c < CH; c++) d += axis[c] * ((float)((P[c][k >> 2] >> (8 * (k & 3))) & 255u) - mean[c]);
+    return d;
+}
+// Endpoints of the line's span [lo, hi], widened to one unit when shorter and clamped to [0,255]; K:882-905.  v[0..3] = A,
+// v[4..7] = B; components >= CH are zero (the reference's never-written slots, rule F6).
+template <int CH>
+ITW_HD Bc7Seg bc7_ends(const Bc7Line& l, float lo, float hi)
+{
+    if (hi - lo < 1.0f) { lo -= 0.5f; hi += 0.5f; }
+    Bc7Seg seg;
+#pragma unroll
+    for (int i = 0; i < 8; i++) seg.v[i] = 0.0f;
+#pragma unroll
+    for (int c = 0; c < CH; c++) {
+        seg.v[c] = clamp_sse(lo * l.axis[c] + l.mean[c], 0.0f, 255.0f);
+        seg.v[4 + c] = clamp_sse(hi * l.axis[c] + l.mean[c], 0.0f, 255.0f);
+    }
+    return seg;
+}
+template <int CH>
+ITW_HD Bc7Seg bc7_fit_impl(const View& v, u32 mask)
+{
+    u32 P[4][4];
+    load_planes(P, v);
+    int st[15];
+    moments_u8(st, P, mask, CH);
+    const Bc7Line l = bc7_line<CH, false>(st);
     float lo = inf_f(), hi = -inf_f();
 #pragma unroll
     for (int k = 0; k < 16; k++) {
-        // the reference starts the sum from 0.0f; 0 + x differs from x only in the sign of a zero, which nothing below can
-        // observe (see the next comment), so the sum starts from the first product
-        float d = axis[0] * ((float)((P[0][k >> 2] >> (8 * (k & 3))) & 255u) - mean[0]);
-#pragma unroll
-        for (int c = 1; c < CH; c++) d += axis[c] * ((float)((P[c][k >> 2] >> (8 * (k & 3))) & 255u) - mean[c]);
+        const float d = bc7_project<CH>(l.axis, l.mean, P, k);
         // d is finite here (8-bit texels, finite axis), so the reference's (a<b)?a:b equals fminf/fmaxf up to
-        // the sign of a zero, which the affine map below cannot observe: one FMNMX instead of FSETP+FSEL
+        // the sign of a zero, which the affine map of bc7_ends cannot observe: one FMNMX instead of FSETP+FSEL
         if ((mask >> k) & 1u) {
             lo = fminf(lo, d);
             hi = fmaxf(hi, d);
         }
     }
-    if (hi - lo < 1.0f) { lo -= 0.5f; hi += 0.5f; }
-#pragma unroll
-    for (int c = 0; c < CH; c++) {
-        ep[c] = clamp_sse(lo * axis[c] + mean[c], 0.0f, 255.0f);
-        ep[4 + c] = clamp_sse(hi * axis[c] + mean[c], 0.0f, 255.0f);
-    }
+    return bc7_ends<CH>(l, lo, hi);
 }
-// PCA line through the masked texels, clamped to [0,255]; K:834-905.  v[0..3] = A, v[4..7] = B;
-// components >= channels are zero (the reference's never-written slots, rule F6).
+// PCA line through the masked texels, clamped to [0,255]; K:834-905.
 ITW_HD_NOINLINE Bc7Seg bc7_fit(const Bc7Block* blk, int rot, int alpha, u32 mask, int channels)
 {
     const View v{blk, rot, alpha};
-    Bc7Seg seg;
-#pragma unroll
-    for (int i = 0; i < 8; i++) seg.v[i] = 0.0f;
-    float unused;
-    if (channels == 4) bc7_fit_impl<4, false>(seg.v, unused, v, mask);
-    else bc7_fit_impl<3, false>(seg.v, unused, v, mask);
-    return seg;
+    return (channels == 4) ? bc7_fit_impl<4>(v, mask) : bc7_fit_impl<3>(v, mask);
 }
 // Both subsets of a two-subset shape of an untransformed block: the same values as bc7_fit of mask0 and of its complement
 // (and, at three channels, their split bounds), with the work the two fits share done once.  Subset 1's integer moments are
-// the block's minus subset 0's (exact); the two covariance / power-iteration chains are independent, so the scheduler can
-// interleave them; one projection loop sends every texel to its own subset's axis and mean.
+// the block's minus subset 0's (exact); the two lines are independent, so the scheduler can interleave them; one projection
+// loop sends every texel to its own subset's line.
 struct Bc7Pair { Bc7Seg seg[2]; float bound[2]; };
-template <int CH, bool kBound>
-ITW_HD void bc7_fit_pair_impl(Bc7Pair& f, const Bc7Block* blk, u32 mask0)
+template <int CH>
+ITW_HD Bc7Pair bc7_fit_pair_impl(const Bc7Block* blk, u32 mask0)
 {
-    static_assert(!kBound || CH == 3, "the four-channel fit adds eps to slot 9, the split bound does not");
     u32 P[4][4];
     load_planes(P, View{blk, 3, 1});
     int full[15], part[15], rest[15];
@@ -384,64 +412,31 @@ ITW_HD void bc7_fit_pair_impl(Bc7Pair& f, const Bc7Block* blk, u32 mask0)
     moments_u8(part, P, mask0, CH);
 #pragma unroll
     for (int i = 0; i < 15; i++) rest[i] = full[i] - part[i];
-    float cov0[10], cov1[10], mean0[4], mean1[4];
-    bc7_covariance<CH>(cov0, mean0, part);
-    bc7_covariance<CH>(cov1, mean1, rest);
-    const float inv_var = 1.0f / (256.0f * 256.0f);
-#pragma unroll
-    for (int i = 0; i < 10; i++) { cov0[i] *= inv_var; cov1[i] *= inv_var; }
-    const float eps = 0.001f * 0.001f;
-    cov0[0] += eps; cov0[4] += eps; cov0[7] += eps; cov0[9] += eps;
-    cov1[0] += eps; cov1[4] += eps; cov1[7] += eps; cov1[9] += eps;
-    float axis0[4] = {1.0f, 1.0f, 1.0f, 1.0f}, axis1[4] = {1.0f, 1.0f, 1.0f, 1.0f};
-    bc7_power_axis<CH, 4>(axis0, cov0);
-    bc7_power_axis<CH, 4>(axis1, cov1);
-    f.bound[0] = f.bound[1] = 0.0f;
-    if (kBound) {
-        f.bound[0] = bc7_bound_from_axis<CH>(cov0, axis0);
-        f.bound[1] = bc7_bound_from_axis<CH>(cov1, axis1);
-    }
-    bc7_power_axis<CH, 4>(axis0, cov0);
-    bc7_power_axis<CH, 4>(axis1, cov1);
-
+    const Bc7Line l0 = bc7_line<CH, CH == 3>(part), l1 = bc7_line<CH, CH == 3>(rest);
     float lo0 = inf_f(), hi0 = -inf_f(), lo1 = inf_f(), hi1 = -inf_f();
 #pragma unroll
     for (int k = 0; k < 16; k++) {
-        // bc7_fit_impl's projection with the texel's own subset's axis and mean: same operands, same order
         const bool in0 = (mask0 >> k) & 1u;
-        float d = (in0 ? axis0[0] : axis1[0]) * ((float)((P[0][k >> 2] >> (8 * (k & 3))) & 255u) - (in0 ? mean0[0] : mean1[0]));
+        float axis[4], mean[4];
 #pragma unroll
-        for (int c = 1; c < CH; c++)
-            d += (in0 ? axis0[c] : axis1[c]) * ((float)((P[c][k >> 2] >> (8 * (k & 3))) & 255u) - (in0 ? mean0[c] : mean1[c]));
+        for (int c = 0; c < 4; c++) { axis[c] = in0 ? l0.axis[c] : l1.axis[c]; mean[c] = in0 ? l0.mean[c] : l1.mean[c]; }
+        const float d = bc7_project<CH>(axis, mean, P, k);
         if (in0) { lo0 = fminf(lo0, d); hi0 = fmaxf(hi0, d); }
         else     { lo1 = fminf(lo1, d); hi1 = fmaxf(hi1, d); }
     }
-    if (hi0 - lo0 < 1.0f) { lo0 -= 0.5f; hi0 += 0.5f; }
-    if (hi1 - lo1 < 1.0f) { lo1 -= 0.5f; hi1 += 0.5f; }
-#pragma unroll
-    for (int i = 0; i < 8; i++) f.seg[0].v[i] = f.seg[1].v[i] = 0.0f;
-#pragma unroll
-    for (int c = 0; c < CH; c++) {
-        f.seg[0].v[c] = clamp_sse(lo0 * axis0[c] + mean0[c], 0.0f, 255.0f);
-        f.seg[0].v[4 + c] = clamp_sse(hi0 * axis0[c] + mean0[c], 0.0f, 255.0f);
-        f.seg[1].v[c] = clamp_sse(lo1 * axis1[c] + mean1[c], 0.0f, 255.0f);
-        f.seg[1].v[4 + c] = clamp_sse(hi1 * axis1[c] + mean1[c], 0.0f, 255.0f);
-    }
+    return Bc7Pair{{bc7_ends<CH>(l0, lo0, hi0), bc7_ends<CH>(l1, lo1, hi1)}, {l0.bound, l1.bound}};
 }
 // mask0 = subset 0 of a two-subset shape; bound[] is set at three channels only
 ITW_HD_NOINLINE Bc7Pair bc7_fit_pair(const Bc7Block* blk, u32 mask0, int channels)
 {
-    Bc7Pair f;
-    if (channels == 4) bc7_fit_pair_impl<4, false>(f, blk, mask0);
-    else bc7_fit_pair_impl<3, true>(f, blk, mask0);
-    return f;
+    return (channels == 4) ? bc7_fit_pair_impl<4>(blk, mask0) : bc7_fit_pair_impl<3>(blk, mask0);
 }
 // Two subset masks of an untransformed block at three channels (a lane pair of the three-subset masks): the same values as
-// bc7_fit(blk, 3, 1, mask, 3) of each.  The masks are not complements, so each has its own moment pass; the two covariance /
-// power-iteration chains are independent, so the scheduler can interleave them; one projection loop converts every texel
-// once and projects it onto both axes.  Inlined into bc7_phase_masks3, like bc7_masks_error2: as non-inlined routines they
-// moved ptxas's register assignment of the shared callees so that bc7_chain spilled 160 bytes instead of 4 to 20
-// (-Xptxas -v), and basic / alpha_basic ran 0.4 / 1.4 % slower on H100.
+// bc7_fit(blk, 3, 1, mask, 3) of each.  The masks are not complements, so each has its own moment pass; the two lines are
+// independent, so the scheduler can interleave them; one projection loop converts every texel once and projects it onto
+// both.  Inlined into bc7_phase_masks3, like bc7_masks_error2: as non-inlined routines they moved ptxas's register
+// assignment of the shared callees so that bc7_chain spilled 160 bytes instead of 4 to 20 (-Xptxas -v), and basic /
+// alpha_basic ran 0.4 / 1.4 % slower on H100.
 struct Bc7Segs2 { Bc7Seg seg[2]; };
 ITW_HD Bc7Segs2 bc7_fit_masks2(const Bc7Block* blk, u32 mask_a, u32 mask_b)
 {
@@ -450,61 +445,22 @@ ITW_HD Bc7Segs2 bc7_fit_masks2(const Bc7Block* blk, u32 mask_a, u32 mask_b)
     int sta[15], stb[15];
     moments_u8(sta, P, mask_a, 3);
     moments_u8(stb, P, mask_b, 3);
-    float cova[10], covb[10], meana[4], meanb[4];
-    bc7_covariance<3>(cova, meana, sta);
-    bc7_covariance<3>(covb, meanb, stb);
-    const float inv_var = 1.0f / (256.0f * 256.0f);
-#pragma unroll
-    for (int i = 0; i < 10; i++) { cova[i] *= inv_var; covb[i] *= inv_var; }
-    const float eps = 0.001f * 0.001f;
-    cova[0] += eps; cova[4] += eps; cova[7] += eps; cova[9] += eps;
-    covb[0] += eps; covb[4] += eps; covb[7] += eps; covb[9] += eps;
-    float axisa[4] = {1.0f, 1.0f, 1.0f, 1.0f}, axisb[4] = {1.0f, 1.0f, 1.0f, 1.0f};
-    bc7_power_axis<3, 4>(axisa, cova);
-    bc7_power_axis<3, 4>(axisb, covb);
-    bc7_power_axis<3, 4>(axisa, cova);
-    bc7_power_axis<3, 4>(axisb, covb);
-
+    const Bc7Line la = bc7_line<3, false>(sta), lb = bc7_line<3, false>(stb);
     float loa = inf_f(), hia = -inf_f(), lob = inf_f(), hib = -inf_f();
 #pragma unroll
     for (int k = 0; k < 16; k++) {
-        // bc7_fit_impl's projection onto each mask's axis and mean: same operands, same order
-        float x[3];
-#pragma unroll
-        for (int c = 0; c < 3; c++) x[c] = (float)((P[c][k >> 2] >> (8 * (k & 3))) & 255u);
-        float da = axisa[0] * (x[0] - meana[0]), db = axisb[0] * (x[0] - meanb[0]);
-#pragma unroll
-        for (int c = 1; c < 3; c++) {
-            da += axisa[c] * (x[c] - meana[c]);
-            db += axisb[c] * (x[c] - meanb[c]);
-        }
+        const float da = bc7_project<3>(la.axis, la.mean, P, k), db = bc7_project<3>(lb.axis, lb.mean, P, k);
         if ((mask_a >> k) & 1u) { loa = fminf(loa, da); hia = fmaxf(hia, da); }
         if ((mask_b >> k) & 1u) { lob = fminf(lob, db); hib = fmaxf(hib, db); }
     }
-    if (hia - loa < 1.0f) { loa -= 0.5f; hia += 0.5f; }
-    if (hib - lob < 1.0f) { lob -= 0.5f; hib += 0.5f; }
-    Bc7Segs2 f;
-#pragma unroll
-    for (int i = 0; i < 8; i++) f.seg[0].v[i] = f.seg[1].v[i] = 0.0f;
-#pragma unroll
-    for (int c = 0; c < 3; c++) {
-        f.seg[0].v[c] = clamp_sse(loa * axisa[c] + meana[c], 0.0f, 255.0f);
-        f.seg[0].v[4 + c] = clamp_sse(hia * axisa[c] + meana[c], 0.0f, 255.0f);
-        f.seg[1].v[c] = clamp_sse(lob * axisb[c] + meanb[c], 0.0f, 255.0f);
-        f.seg[1].v[4 + c] = clamp_sse(hib * axisb[c] + meanb[c], 0.0f, 255.0f);
-    }
-    return f;
+    return Bc7Segs2{{bc7_ends<3>(la, loa, hia), bc7_ends<3>(lb, lob, hib)}};
 }
 
-// trace - lambda_max of a covariance; K:907-939 (eps on three diagonal slots only, K:918-920)
+// trace - lambda_max of a covariance after four power iterations; K:907-939
 template <int CH>
 ITW_HD float bc7_residual_bound(float (&cov)[10])
 {
-    const float inv_var = 1.0f / (256.0f * 256.0f);
-#pragma unroll
-    for (int i = 0; i < 10; i++) cov[i] *= inv_var;
-    const float eps = 0.001f * 0.001f;
-    cov[0] += eps; cov[4] += eps; cov[7] += eps;
+    bc7_scale_covariance<false>(cov);
     float axis[4] = {1.0f, 1.0f, 1.0f, 1.0f};
     bc7_power_axis<CH, 4>(axis, cov);
     return bc7_bound_from_axis<CH>(cov, axis);
@@ -651,6 +607,79 @@ ITW_HD Bc7Lerp bc7_lerp(u32 a, u32 b)
     const u32 a_rb = a & m, a_ga = (a >> 8) & m;
     return Bc7Lerp{(a_rb << 6) + 0x00200020u, (a_ga << 6) + 0x00200020u, (b & m) - a_rb, ((b >> 8) & m) - a_ga};
 }
+// Per-subset constants of a search with endpoints a, b (channels that do not take part already zeroed): the numerator offset
+// cj = a.(b - a) and the squared length idiv = |b - a|^2, exact integers, and the palette interpolation.
+struct Bc7Sub { u32 a, b; int cj, idiv; Bc7Lerp lerp; };
+ITW_HD Bc7Sub bc7_sub(u32 a, u32 b)
+{
+    const u32 aa = dp4a_u8(a, a, 0u), ab = dp4a_u8(a, b, 0u), bb = dp4a_u8(b, b, 0u);
+    return Bc7Sub{a, b, (int)(ab - aa), (int)(bb - 2u * ab + aa), bc7_lerp(a, b)};
+}
+// Projection numerator of texel t, sum_c (t_c - a_c)(b_c - a_c): an integer, |value| < 2^18, so the float it converts to is
+// the reference's float sum (K:1148-1156)
+ITW_HD int bc7_num(u32 t, u32 a, u32 b, int cj) { return (int)dp4a_u8(t, b, 0u) - (int)dp4a_u8(t, a, 0u) - cj; }
+// q1 by the quotient num / div of K:1158, evaluated as the exact FMA-corrected quotient (proved equal to IEEE num/div on this
+// integer domain, tests/test_exact_division.py).  |proj*levels| < 2^23, so truncation never overflows; NaN (coincident
+// endpoints, 0/0) becomes INT_MIN on x86 and 0 here -- both clamp to 1 (K:1160-1161).  proj*levels is exact, so the fused
+// form rounds once like the reference's multiply-then-add.
+ITW_HD int bc7_q1_quotient(int num, float fdiv, float rdiv, float flevels, int levels)
+{
+    const float proj = div_by_rcp((float)num, fdiv, rdiv);
+    return clampi(trunc_i(fma_rn(proj, flevels, 0.5f)), 1, levels - 1);
+}
+// Two-bit search by thresholds: q1 = 1 + (num >= t2) + (num >= t3), t2 <= t3.  The reference's
+// q1 = clamp((int)(RN(RN(num / div) * 4) + 0.5), 1, 3) is a non-decreasing step function of the integer num; with
+// tau = (2m - 1) / 8 (a float): RN(p * 4 + 0.5) >= m <=> p >= tau (the sum is exact below the next binade, and the binade
+// boundary itself is an integer m), and RN(num / div) >= tau <=> num / div >= tau because a quotient below tau stays at
+// least 1 / (8 div) > 2^-21 away from it while half an ulp of tau is below 2^-24 (div <= 4 * 255^2 < 2^18).  So
+// q1 >= m  <=>  8 num >= (2m - 1) div  <=>  num >= ceil((2m - 1) div / 8), m = 2, 3; coincident endpoints give 0/0 = NaN ->
+// q1 = 1 in the reference: thresholds out of reach.  tests/test_exact_division.py checks both sides of every step for every
+// possible div.
+struct Bc7Thresholds { int t2, t3; };
+ITW_HD Bc7Thresholds bc7_thresholds(int idiv)
+{
+    return Bc7Thresholds{idiv ? (3 * idiv + 7) >> 3 : 0x7fffffff, idiv ? (5 * idiv + 7) >> 3 : 0x7fffffff};
+}
+struct Bc7Steps {
+    bool ge2, ge3;
+    ITW_HD int q1() const { return 1 + (ge2 ? 1 : 0) + (ge3 ? 1 : 0); }
+};
+ITW_HD Bc7Steps bc7_steps(int num, int t2, int t3) { return Bc7Steps{num >= t2, num >= t3}; }
+// The better of palette entries q1 - 1 (`lo`) and q1 (`hi`) for texel t: VABSDIFF4 + IDP.4A errors, q1 on a tie (K:1163-1184)
+struct Bc7Pick { int err; bool first; };
+ITW_HD Bc7Pick bc7_pick(u32 lo, u32 hi, u32 t)
+{
+    const u32 d0 = absdiff_u8x4(lo, t), d1 = absdiff_u8x4(hi, t);
+    const int e0 = (int)dp4a_u8(d0, d0, 0u), e1 = (int)dp4a_u8(d1, d1, 0u);
+    const bool first = e0 < e1;
+    return Bc7Pick{first ? e0 : e1, first};
+}
+// bc7_assign's texel loop: palette and per-subset constants from lane-private shared memory.  kThresholds: the two-bit
+// search by thresholds; kIdentity: the texel words are read as stored (every shape-phase search, the partitioned and mode-6
+// chains), else through the rotated view (modes 4 / 5).  Separate instantiations, not a branch inside the loop.
+template <bool kThresholds, bool kIdentity>
+ITW_HD Bc7Search bc7_assign_texels(const u32 (*pal)[32], int lane, const View& v, int levels, u32 pattern, u32 chmask)
+{
+    const u32* tx = (chmask == 0x00FFFFFFu) ? v.b->rgb : v.b->tex;
+    const int lv = kThresholds ? 4 : levels;
+    const float flevels = (float)levels;
+    int total = 0;
+    u32 out0 = 0u, out1 = 0u;
+    ITW_UNROLL(ITW_BC7_ASSIGN_UNROLL)
+    for (int k = 0; k < 16; k++) {
+        const u32 t = kIdentity ? tx[k] : (view_tex(v, k) & chmask);
+        const int j = (int)((pattern >> (2 * k)) & 3u);
+        const int num = bc7_num(t, pal[24 + 5 * j + 0][lane], pal[24 + 5 * j + 1][lane], (int)pal[24 + 5 * j + 2][lane]);
+        const int q1 = kThresholds ? bc7_steps(num, (int)pal[24 + 5 * j + 3][lane], (int)pal[24 + 5 * j + 4][lane]).q1()
+                                   : bc7_q1_quotient(num, bits_float(pal[24 + 5 * j + 3][lane]), bits_float(pal[24 + 5 * j + 4][lane]),
+                                                     flevels, levels);
+        const Bc7Pick p = bc7_pick(pal[j * lv + q1 - 1][lane], pal[j * lv + q1][lane], t);
+        total += p.err;
+        const u32 bq = (u32)(p.first ? q1 - 1 : q1) << (4 * (k & 7));
+        if (k < 8) out0 += bq; else out1 += bq;
+    }
+    return Bc7Search{total, out0, out1};
+}
 ITW_HD_NOINLINE Bc7Search bc7_assign(u32 (*pal)[32], int lane, const Bc7Block* blk, int rot, int alpha, int bits_flags, int pairs,
                                      u32 pattern, u32 e0, u32 e1, u32 e2, u32 e3, u32 e4, u32 e5, u32 chmask)
 {
@@ -662,145 +691,56 @@ ITW_HD_NOINLINE Bc7Search bc7_assign(u32 (*pal)[32], int lane, const Bc7Block* b
     // loop: the load/store pipe is nearly idle in this kernel while the ALU pipe (selects) is the busiest
     u32 cur_a = e0, cur_b = e1, next_a = e2, next_b = e3;        // endpoints walk through two register pairs: no select by j
     for (int j = 0; j < pairs; j++) {
-        const u32 a = cur_a & chmask, b = cur_b & chmask;
+        const Bc7Sub s = bc7_sub(cur_a & chmask, cur_b & chmask);
         cur_a = next_a; cur_b = next_b; next_a = e4; next_b = e5;
-        const u32 aa = dp4a_u8(a, a, 0u), ab = dp4a_u8(a, b, 0u), bb = dp4a_u8(b, b, 0u);
-        const int idiv = (int)(bb - 2u * ab + aa);               // sum of squared differences, exact
-        pal[24 + 5 * j + 0][lane] = a;
-        pal[24 + 5 * j + 1][lane] = b;
-        pal[24 + 5 * j + 2][lane] = ab - aa;
+        pal[24 + 5 * j + 0][lane] = s.a;
+        pal[24 + 5 * j + 1][lane] = s.b;
+        pal[24 + 5 * j + 2][lane] = (u32)s.cj;
         if (thresholds) {
-            // two-bit search by thresholds: q1 >= m  <=>  8 num >= (2m - 1) div  <=>  num >= ceil((2m - 1) div / 8), m = 2, 3
-            // (see the texel loop); coincident endpoints give 0/0 = NaN -> q1 = 1 in the reference: thresholds out of reach
-            pal[24 + 5 * j + 3][lane] = (u32)(idiv ? (3 * idiv + 7) >> 3 : 0x7fffffff);
-            pal[24 + 5 * j + 4][lane] = (u32)(idiv ? (5 * idiv + 7) >> 3 : 0x7fffffff);
+            const Bc7Thresholds th = bc7_thresholds(s.idiv);
+            pal[24 + 5 * j + 3][lane] = (u32)th.t2;
+            pal[24 + 5 * j + 4][lane] = (u32)th.t3;
         } else {
-            const float fdiv = (float)idiv;
+            const float fdiv = (float)s.idiv;
             pal[24 + 5 * j + 3][lane] = float_bits(fdiv);
-            pal[24 + 5 * j + 4][lane] = float_bits(1.0f / fdiv);  // inf when the endpoints coincide (-> NaN below, as 0/0)
+            pal[24 + 5 * j + 4][lane] = float_bits(1.0f / fdiv);  // inf when the endpoints coincide (-> NaN, as 0/0)
         }
-        const Bc7Lerp lerp = bc7_lerp(a, b);
-        pal[j * levels][lane] = a;
-        pal[j * levels + levels - 1][lane] = b;
-        for (int q = 1; q < levels - 1; q++) pal[j * levels + q][lane] = lerp.entry((u32)bc7_weight(bits, q));
+        pal[j * levels][lane] = s.a;
+        pal[j * levels + levels - 1][lane] = s.b;
+        for (int q = 1; q < levels - 1; q++) pal[j * levels + q][lane] = s.lerp.entry((u32)bc7_weight(bits, q));
     }
-    const float flevels = (float)levels;
-    int total = 0;
-    u32 out0 = 0u, out1 = 0u;
-    if (thresholds) {
-        // The reference's q1 = clamp((int)(RN(RN(num / div) * 4) + 0.5), 1, 3) is a non-decreasing step function of the
-        // integer num; with tau = (2m - 1) / 8 (a float): RN(p * 4 + 0.5) >= m <=> p >= tau (the sum is exact below the next
-        // binade, and the binade boundary itself is an integer m), and RN(num / div) >= tau <=> num / div >= tau because a
-        // quotient below tau stays at least 1 / (8 div) > 2^-21 away from it while half an ulp of tau is below 2^-24
-        // (div <= 4 * 255^2 < 2^18).  tests/test_exact_division.py checks both sides of every step for every possible div.
-        const u32* tx = (chmask == 0x00FFFFFFu) ? blk->rgb : blk->tex;
-        ITW_UNROLL(ITW_BC7_ASSIGN_UNROLL)
-        for (int k = 0; k < 16; k++) {
-            const u32 t = tx[k];
-            const int j = (int)((pattern >> (2 * k)) & 3u);
-            const u32 ea = pal[24 + 5 * j + 0][lane], eb = pal[24 + 5 * j + 1][lane];
-            const int cj = (int)pal[24 + 5 * j + 2][lane];
-            const int t2 = (int)pal[24 + 5 * j + 3][lane], t3 = (int)pal[24 + 5 * j + 4][lane];
-            const int num = (int)dp4a_u8(t, eb, 0u) - (int)dp4a_u8(t, ea, 0u) - cj;
-            const int q1 = 1 + ((num >= t2) ? 1 : 0) + ((num >= t3) ? 1 : 0);
-            const u32 p0 = pal[j * 4 + q1 - 1][lane], p1 = pal[j * 4 + q1][lane];
-            const u32 d0 = absdiff_u8x4(p0, t), d1 = absdiff_u8x4(p1, t);
-            const int e0 = (int)dp4a_u8(d0, d0, 0u), e1 = (int)dp4a_u8(d1, d1, 0u);
-            const bool first = e0 < e1;
-            total += first ? e0 : e1;
-            const u32 bq = (u32)(first ? q1 - 1 : q1) << (4 * (k & 7));
-            if (k < 8) out0 += bq; else out1 += bq;
-        }
-    } else
-    if (rot == 3) {
-        // identity view (every shape-phase search, the partitioned and mode-6 chains): the texel words are read as stored
-        const u32* tx = (chmask == 0x00FFFFFFu) ? blk->rgb : blk->tex;
-        ITW_UNROLL(ITW_BC7_ASSIGN_UNROLL)
-        for (int k = 0; k < 16; k++) {
-            const u32 t = tx[k];
-            const int j = (int)((pattern >> (2 * k)) & 3u);
-            const u32 ea = pal[24 + 5 * j + 0][lane], eb = pal[24 + 5 * j + 1][lane];
-            const int cj = (int)pal[24 + 5 * j + 2][lane];
-            const float dj = bits_float(pal[24 + 5 * j + 3][lane]), rj = bits_float(pal[24 + 5 * j + 4][lane]);
-            // sum_c (t_c - a_c)(b_c - a_c): integer, |value| < 2^18, so the float it converts to is the
-            // reference's float sum; the division of K:1158 is the exact FMA-corrected quotient (proved
-            // equal to IEEE num/div on this integer domain, tests/test_exact_division.py)
-            const int num = (int)dp4a_u8(t, eb, 0u) - (int)dp4a_u8(t, ea, 0u) - cj;
-            const float proj = div_by_rcp((float)num, dj, rj);
-            // |proj*levels| < 2^23, so truncation never overflows; NaN (coincident endpoints, 0/0) becomes
-            // INT_MIN on x86 and 0 here -- both clamp to 1 (K:1160-1161).  proj*levels is exact, so the fused
-            // form rounds once like the reference's multiply-then-add.
-            const int q1 = clampi(trunc_i(fma_rn(proj, flevels, 0.5f)), 1, levels - 1);
-            const u32 p0 = pal[j * levels + q1 - 1][lane], p1 = pal[j * levels + q1][lane];
-            const u32 d0 = absdiff_u8x4(p0, t), d1 = absdiff_u8x4(p1, t);
-            const int e0 = (int)dp4a_u8(d0, d0, 0u), e1 = (int)dp4a_u8(d1, d1, 0u);
-            const bool first = e0 < e1;
-            total += first ? e0 : e1;
-            const u32 bq = (u32)(first ? q1 - 1 : q1) << (4 * (k & 7));
-            if (k < 8) out0 += bq; else out1 += bq;
-        }
-    } else {                                                       // rotated views of modes 4 / 5: same loop, texels through view_tex
-        ITW_UNROLL(ITW_BC7_ASSIGN_UNROLL)
-        for (int k = 0; k < 16; k++) {
-            const u32 t = view_tex(v, k) & chmask;
-            const int j = (int)((pattern >> (2 * k)) & 3u);
-            const u32 ea = pal[24 + 5 * j + 0][lane], eb = pal[24 + 5 * j + 1][lane];
-            const int cj = (int)pal[24 + 5 * j + 2][lane];
-            const float dj = bits_float(pal[24 + 5 * j + 3][lane]), rj = bits_float(pal[24 + 5 * j + 4][lane]);
-            const int num = (int)dp4a_u8(t, eb, 0u) - (int)dp4a_u8(t, ea, 0u) - cj;
-            const float proj = div_by_rcp((float)num, dj, rj);
-            const int q1 = clampi(trunc_i(fma_rn(proj, flevels, 0.5f)), 1, levels - 1);
-            const u32 p0 = pal[j * levels + q1 - 1][lane], p1 = pal[j * levels + q1][lane];
-            const u32 d0 = absdiff_u8x4(p0, t), d1 = absdiff_u8x4(p1, t);
-            const int e0 = (int)dp4a_u8(d0, d0, 0u), e1 = (int)dp4a_u8(d1, d1, 0u);
-            const bool first = e0 < e1;
-            total += first ? e0 : e1;
-            const u32 bq = (u32)(first ? q1 - 1 : q1) << (4 * (k & 7));
-            if (k < 8) out0 += bq; else out1 += bq;
-        }
-    }
-    return Bc7Search{total, out0, out1};
+    if (thresholds) return bc7_assign_texels<true, true>(pal, lane, v, levels, pattern, chmask);
+    if (rot == 3) return bc7_assign_texels<false, true>(pal, lane, v, levels, pattern, chmask);
+    return bc7_assign_texels<false, false>(pal, lane, v, levels, pattern, chmask);
 }
-// Shape-phase searches without index bits (three channels, untransformed block): bc7_assign's arithmetic -- the
-// integer-threshold two-bit form, the FMA-corrected quotient for three bits, VABSDIFF4 + IDP.4A errors -- with each subset's
-// constants and palette in registers.  The error of a shape is the sum of the errors of its subsets (exact integers); the
-// first-of-two choice adds min(e0, e1).
-// Two-bit constants of one subset: q1 = 1 + (num >= t2) + (num >= t3), t2 <= t3 (thresholds as in bc7_assign)
+// Shape-phase searches without index bits (three channels, untransformed block): bc7_assign's texel step with each subset's
+// constants and palette in registers.  The error of a shape is the sum of the errors of its subsets (exact integers).
+// Two-bit constants of one subset (thresholds as in bc7_assign)
 struct Bc7Sub2 { u32 a, b; int cj, t2, t3; u32 p1, p2; };
 ITW_HD Bc7Sub2 bc7_sub2(u32 dec_a, u32 dec_b)
 {
-    const u32 a = dec_a & 0x00FFFFFFu, b = dec_b & 0x00FFFFFFu;
-    const u32 aa = dp4a_u8(a, a, 0u), ab = dp4a_u8(a, b, 0u), bb = dp4a_u8(b, b, 0u);
-    const int idiv = (int)(bb - 2u * ab + aa);
-    const Bc7Lerp lerp = bc7_lerp(a, b);
-    return Bc7Sub2{a, b, (int)(ab - aa), idiv ? (3 * idiv + 7) >> 3 : 0x7fffffff, idiv ? (5 * idiv + 7) >> 3 : 0x7fffffff,
-                   lerp.entry((u32)bc7_weight(2, 1)), lerp.entry((u32)bc7_weight(2, 2))};
+    const Bc7Sub s = bc7_sub(dec_a & 0x00FFFFFFu, dec_b & 0x00FFFFFFu);
+    const Bc7Thresholds th = bc7_thresholds(s.idiv);
+    return Bc7Sub2{s.a, s.b, s.cj, th.t2, th.t3, s.lerp.entry((u32)bc7_weight(2, 1)), s.lerp.entry((u32)bc7_weight(2, 2))};
 }
 ITW_HD int bc7_texel_error2(const Bc7Sub2& s, u32 t)
 {
-    const int num = (int)dp4a_u8(t, s.b, 0u) - (int)dp4a_u8(t, s.a, 0u) - s.cj;
-    const bool ge2 = num >= s.t2, ge3 = num >= s.t3;
-    const u32 lo = ge3 ? s.p2 : (ge2 ? s.p1 : s.a), hi = ge3 ? s.b : (ge2 ? s.p2 : s.p1);      // palette entries q1 - 1, q1
-    const u32 d0 = absdiff_u8x4(lo, t), d1 = absdiff_u8x4(hi, t);
-    return mini((int)dp4a_u8(d0, d0, 0u), (int)dp4a_u8(d1, d1, 0u));
+    const Bc7Steps q = bc7_steps(bc7_num(t, s.a, s.b, s.cj), s.t2, s.t3);
+    const u32 lo = q.ge3 ? s.p2 : (q.ge2 ? s.p1 : s.a), hi = q.ge3 ? s.b : (q.ge2 ? s.p2 : s.p1);      // entries q1 - 1, q1
+    return bc7_pick(lo, hi, t).err;
 }
 // Three-bit constants of one subset
 struct Bc7Sub3 { u32 a, b; int cj; float fdiv, rdiv; Bc7Lerp lerp; };
 ITW_HD Bc7Sub3 bc7_sub3(u32 dec_a, u32 dec_b)
 {
-    const u32 a = dec_a & 0x00FFFFFFu, b = dec_b & 0x00FFFFFFu;
-    const u32 aa = dp4a_u8(a, a, 0u), ab = dp4a_u8(a, b, 0u), bb = dp4a_u8(b, b, 0u);
-    const float fdiv = (float)(int)(bb - 2u * ab + aa);
-    return Bc7Sub3{a, b, (int)(ab - aa), fdiv, 1.0f / fdiv, bc7_lerp(a, b)};
+    const Bc7Sub s = bc7_sub(dec_a & 0x00FFFFFFu, dec_b & 0x00FFFFFFu);
+    const float fdiv = (float)s.idiv;
+    return Bc7Sub3{s.a, s.b, s.cj, fdiv, 1.0f / fdiv, s.lerp};
 }
 ITW_HD int bc7_texel_error3(const Bc7Sub3& s, u32 t)
 {
-    const int num = (int)dp4a_u8(t, s.b, 0u) - (int)dp4a_u8(t, s.a, 0u) - s.cj;
-    const float proj = div_by_rcp((float)num, s.fdiv, s.rdiv);
-    const int q1 = clampi(trunc_i(fma_rn(proj, 8.0f, 0.5f)), 1, 7);
-    const u32 lo = s.lerp.entry((u32)bc7_weight(3, q1 - 1)), hi = s.lerp.entry((u32)bc7_weight(3, q1));
-    const u32 d0 = absdiff_u8x4(lo, t), d1 = absdiff_u8x4(hi, t);
-    return mini((int)dp4a_u8(d0, d0, 0u), (int)dp4a_u8(d1, d1, 0u));
+    const int q1 = bc7_q1_quotient(bc7_num(t, s.a, s.b, s.cj), s.fdiv, s.rdiv, 8.0f, 8);
+    return bc7_pick(s.lerp.entry((u32)bc7_weight(3, q1 - 1)), s.lerp.entry((u32)bc7_weight(3, q1)), t).err;
 }
 // Mode-2 errors of the two subset masks of a lane pair: a subset's endpoints depend on its mask alone, so the three-subset
 // phases search every distinct mask once.  One counted loop walks the set bits of both masks, so that the two error chains
@@ -1258,44 +1198,46 @@ ITW_HD_NOINLINE Bc7Result bc7_chain(Bc7Warp& W, const Bc7Params& P, int lane, in
 // =============================================================================================
 ITW_HD int bc7_group_count(const Bc7Warp& W, int g) { return mini(maxi(W.nvalid - kBc7Slots * g, 0), kBc7Slots); }   // valid blocks of group g
 
+// texel k (RGBA8) of block `id` of a surface, blocks in row-major order
+ITW_HD const uint8_t* bc7_texel_ptr(const SurfaceView& s, long long id, int k)
+{
+    const int bw = s.width >> 2;
+    const int by = (int)(id / bw), bx = (int)(id - (long long)by * bw);
+    return s.ptr + (size_t)(by * 4 + (k >> 2)) * (size_t)s.stride + (size_t)(bx * 4 + (k & 3)) * 4;
+}
+// texel k of block `id` of a surface into b.rgb[k] and b.tex[k]
+ITW_HD void bc7_fetch_texel(Bc7Block& b, const SurfaceView& s, long long id, int k)
+{
+    const uint8_t* p = bc7_texel_ptr(s, id, k);
+    const u32 rgb = (u32)p[0] | ((u32)p[1] << 8) | ((u32)p[2] << 16);
+    b.rgb[k] = rgb;
+    b.tex[k] = rgb | ((u32)p[3] << 24);
+}
 // Loads half `half` (blocks 8*half .. 8*half+7 of the round's `ntotal`) into blk[].
 ITW_HD void bc7_phase_load(int lane, Bc7Warp& W, const SurfaceView& s, long long first_block, int ntotal, int half)
 {
-    const int bw = s.width >> 2;
     const int nvalid = mini(maxi(ntotal - kBc7Batch * half, 0), kBc7Batch);
     for (int t = lane; t < nvalid * 16; t += 32) {
-        const int slot = t >> 4, k = t & 15;
-        const long long id = first_block + kBc7Batch * half + slot;
-        const int by = (int)(id / bw), bx = (int)(id - (long long)by * bw);
-        const uint8_t* p = s.ptr + (size_t)(by * 4 + (k >> 2)) * (size_t)s.stride + (size_t)(bx * 4 + (k & 3)) * 4;
-        const u32 rgb = (u32)p[0] | ((u32)p[1] << 8) | ((u32)p[2] << 16);
-        W.blk[slot].rgb[k] = rgb;
-        W.blk[slot].tex[k] = rgb | ((u32)p[3] << 24);
+        const int slot = t >> 4;
+        bc7_fetch_texel(W.blk[slot], s, first_block + kBc7Batch * half + slot, t & 15);
     }
     if (lane == 0) { W.nvalid = nvalid; W.half = half; W.ntotal = ntotal; W.nparked = 0; }
     for (int t = lane; t < kBc7Batch * 5; t += 32) W.win_shape[kBc7Batch * half + t / 5][t % 5] = -1;
 }
 // After the shape phases of the second half: the first half is read again (texels and channel planes) for the chain phase.
+// The plane words are read here too: a transpose after a barrier (bc7_phase_planes) would add a phase.
 ITW_HD void bc7_phase_park(int lane, Bc7Warp& W, const SurfaceView& s, long long first_block, int ntotal)
 {
     if (ntotal <= kBc7Batch) return;                       // single-half round: blk[] still holds it
-    const int bw = s.width >> 2;
     for (int t = lane; t < kBc7Batch * 16; t += 32) {
         const int slot = t >> 4, k = t & 15;
         const long long id = first_block + slot;
-        const int by = (int)(id / bw), bx = (int)(id - (long long)by * bw);
-        const uint8_t* p = s.ptr + (size_t)(by * 4 + (k >> 2)) * (size_t)s.stride + (size_t)(bx * 4 + (k & 3)) * 4;
-        const u32 rgb = (u32)p[0] | ((u32)p[1] << 8) | ((u32)p[2] << 16);
-        W.parked[slot].rgb[k] = rgb;
-        W.parked[slot].tex[k] = rgb | ((u32)p[3] << 24);
+        bc7_fetch_texel(W.parked[slot], s, id, k);
         // plane word (c, i) = channel c of texels 4i..4i+3: here c = k & 3, i = k >> 2 (any bijection of 16 onto (c, i) does)
         const int c = k & 3, i = k >> 2;
         u32 v = 0;
 #pragma unroll
-        for (int j = 0; j < 4; j++) {
-            const int kk = 4 * i + j;
-            v |= (u32)s.ptr[(size_t)(by * 4 + (kk >> 2)) * (size_t)s.stride + (size_t)(bx * 4 + (kk & 3)) * 4 + c] << (8 * j);
-        }
+        for (int j = 0; j < 4; j++) v |= (u32)bc7_texel_ptr(s, id, 4 * i + j)[c] << (8 * j);
         W.parked[slot].plane[c][i] = v;
     }
     if (lane == 0) W.nparked = kBc7Batch;

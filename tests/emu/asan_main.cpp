@@ -42,8 +42,8 @@ int main()
             emu_CompressBlocksBC3(&s8, out.data());
             emu_CompressBlocksBC4(&s8, out.data());
             emu_CompressBlocksBC5(&s8, out.data());
-            for (int per_warp = 8; per_warp <= 16; per_warp += 8) {
-                emu_set_bc7_per_warp(per_warp);
+            for (int per_warp = 1; per_warp <= 16; per_warp *= 2) {
+                if (emu_set_bc7_per_warp(per_warp) != 0) return 1;
                 for (int row = 0; row < 10; row++) {
                     bc7_enc_settings st;
                     bc7_fill_profile(&st, row);

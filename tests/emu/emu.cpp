@@ -70,8 +70,15 @@ void emu_set_lane_order(int mode) { g_lane_order = mode; }
 static inline int emu_lane(int i) { return g_lane_order == 0 ? i : (g_lane_order == 1 ? 31 - i : (int)((i * 13u + 7u) & 31u)); }
 #define ITW_PHASE_EMU(call) for (int lane_i = 0; lane_i < 32; lane_i++) { const int lane = emu_lane(lane_i); call; }
 
+// Blocks per warp and round: bc7_kernel runs 16 in a full round and 1, 2, 4, 8 or 16 in the last one; the emulation runs
+// a whole surface in rounds of one such size.  Returns -1 (and keeps the setting) for any other count.
 static int g_bc7_per_warp = kBc7Super;
-void emu_set_bc7_per_warp(int n) { g_bc7_per_warp = (n == kBc7Batch) ? kBc7Batch : kBc7Super; }   // what the host picks by surface size
+int emu_set_bc7_per_warp(int n)
+{
+    if (n != 1 && n != 2 && n != 4 && n != 8 && n != 16) return -1;
+    g_bc7_per_warp = n;
+    return 0;
+}
 void emu_CompressBlocksBC7(const rgba_surface* src, uint8_t* dst, bc7_enc_settings* settings)
 {
     SurfaceView surf = view_of(src);

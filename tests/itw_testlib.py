@@ -69,14 +69,19 @@ def ref_frontend():
     return lib
 
 
-@functools.lru_cache(None)
-def emu():
+def build_emu():
+    """tests/emu/build_emu.py: the CPU build of the kernel logic (its g++ flags and compile())."""
     sys.path.insert(0, os.path.join(ROOT, "tests", "emu"))
     try:
         import build_emu
-        build_emu.build(verbose=False)
     finally:
         sys.path.pop(0)
+    return build_emu
+
+
+@functools.lru_cache(None)
+def emu():
+    build_emu().build(verbose=False)
     return binding.EncoderApi(EMU_SO, "emu_")
 
 

@@ -6,12 +6,10 @@ import ctypes
 import importlib.util
 import os
 import re
-import subprocess
 
 import itw_testlib as T
 import test_bc7_pair_fit as pair_fit
 
-SRC = os.path.join(T.ROOT, "tests", "emu", "mask3_pair_check.cpp")
 MASKS3 = os.path.join(T.ROOT, "intel-texture-works-plugin_b200", "csrc", "itw_masks3.cuh")
 
 
@@ -66,10 +64,7 @@ def test_mask3_table_is_generated_and_paired():
 
 
 def test_mask_pair_routines_equal_per_mask_routines(tmp_path):
-    lib = str(tmp_path / "mask3_pair_check.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-fPIC", "-shared", "-ffp-contract=off", "-fno-fast-math", "-fwrapv",
-                           "-mfpmath=sse", "-msse2", "-Wno-unknown-pragmas", SRC, "-o", lib])
-    dll = ctypes.CDLL(lib)
+    dll = pair_fit.check_lib(tmp_path)
     assert dll.mask3_pair_count() == 70
     check = dll.mask3_pair_check
     check.restype = ctypes.c_int

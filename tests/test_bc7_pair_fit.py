@@ -1,16 +1,20 @@
 """The BC7 shape phases fit both subsets of a two-subset shape in one routine (bc7_fit_pair) and score both of its mode-1 and
 mode-3 searches in one texel walk (bc7_pair_error).  Compiled for the CPU like the emulation, every output must equal the
-per-subset routines -- bc7_fit, the split bound and key of the ranking, bc7_assign -- over all 64 shapes, on random blocks
-and on blocks with ties and flat subsets."""
+per-subset routines -- bc7_fit, a split bound written out in the driver and the key of the ranking, bc7_assign -- over all
+64 shapes, on random blocks and on blocks with ties and flat subsets."""
 import ctypes
 import os
-import subprocess
 
 import numpy as np
 
 import itw_testlib as T
 
-SRC = os.path.join(T.ROOT, "tests", "emu", "pair_fit_check.cpp")
+SRC = os.path.join(T.ROOT, "tests", "emu", "bc7_pair_check.cpp")
+
+
+def check_lib(tmp_path):
+    """tests/emu/bc7_pair_check.cpp, compiled for the CPU like the emulation."""
+    return ctypes.CDLL(T.build_emu().compile_cpu(SRC, str(tmp_path / "bc7_pair_check.so")))
 
 
 def blocks():
@@ -31,10 +35,7 @@ def blocks():
 
 
 def test_pair_fit_equals_per_subset_routines(tmp_path):
-    lib = str(tmp_path / "pair_fit_check.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-fPIC", "-shared", "-ffp-contract=off", "-fno-fast-math", "-fwrapv",
-                           "-mfpmath=sse", "-msse2", "-Wno-unknown-pragmas", SRC, "-o", lib])
-    check = ctypes.CDLL(lib).pair_fit_check
+    check = check_lib(tmp_path).pair_fit_check
     check.restype = ctypes.c_int
     tex = blocks()
     what = ctypes.create_string_buffer(256)

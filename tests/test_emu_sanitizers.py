@@ -5,15 +5,16 @@ import os
 import subprocess
 import tempfile
 
+import itw_testlib as T
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 def test_kernel_logic_under_asan_and_ubsan():
     with tempfile.TemporaryDirectory() as tmp:
         exe = os.path.join(tmp, "emu_asan")
-        subprocess.check_call(["g++", "-std=c++17", "-O1", "-g", "-fsanitize=address,undefined", "-fno-sanitize-recover=undefined",
-                               "-ffp-contract=off", "-fno-fast-math", "-fwrapv", "-mfpmath=sse", "-msse2", "-Wno-unknown-pragmas",
-                               os.path.join(HERE, "emu", "asan_main.cpp"), "-o", exe])
+        T.build_emu().compile_cpu(os.path.join(HERE, "emu", "asan_main.cpp"), exe,
+                                  ["-O1", "-g", "-fsanitize=address,undefined", "-fno-sanitize-recover=undefined"])
         env = dict(os.environ, ASAN_OPTIONS="detect_leaks=0:abort_on_error=1", UBSAN_OPTIONS="print_stacktrace=1:halt_on_error=1")
         res = subprocess.run([exe], capture_output=True, text=True, env=env, timeout=1200)
     assert res.returncode == 0, res.stderr[-3000:]
