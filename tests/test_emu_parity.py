@@ -33,9 +33,9 @@ def test_ragged_batches_and_strides(fmt, prof):
 @pytest.mark.parametrize("per_warp", [8, 16])
 @pytest.mark.parametrize("prof", ["slow", "alpha_slow", "alpha_fast", "veryfast"])
 def test_bc7_round_sizes(prof, per_warp):
-    """The BC7 warp program in rounds of 16 blocks (two halves, one chain phase: every full round) and of 8 (one half: a last
-    round), with every ragged remainder 1..17 of the surface's last round, equals the oracle (test_bc7_emu_per_warp.py runs
-    every count on tie-heavy blocks)."""
+    """The BC7 warp program with 16 blocks per warp (two halves, one chain phase: every full round, and a last round dealt 16
+    per warp) and with 8 (one half: a last round dealt 8 per warp), with every ragged remainder 1..17 of the surface's last
+    round, equals the oracle (test_bc7_emu_per_warp.py runs every count 1, 2, 4, 8 and 16 on tie-heavy blocks)."""
     import ctypes
     emu = T.emu()
     setter = emu.lib.emu_set_bc7_per_warp

@@ -106,9 +106,12 @@ def test_unaligned_source_pointer():
 
 @pytest.mark.parametrize("prof", ["veryfast", "alpha_fast"])
 def test_bc7_sixteen_block_rounds_ragged_and_unaligned(prof):
-    """Surfaces with at least SMs x 16 x 16 blocks (33 792 on a 132-SM H100) run BC7 in rounds of sixteen blocks per warp (two halves, one chain phase;
-    smaller ones keep eight): a block count that fills neither the last round nor the last CTA tile, through the TMA-staged
-    kernel and -- from a source address that is not 16-byte aligned -- through the plain-load kernel, against the oracle."""
+    """A launch runs BC7 in full rounds of sixteen blocks per warp (SMs x 16 x 16 blocks, 33 792 on a 132-SM H100); the blocks
+    left over are dealt over all warps of the grid as one last round of 1, 2, 4, 8 or 16 per warp.  A host surface of 65 535
+    blocks goes through the band pipeline (four launches of whole block rows, each ending in such a last round with a ragged
+    last warp and CTA tile), from a host source that is 16-byte aligned and from one that is not, against the oracle.  The
+    bands are staged into tight device rows, so both take the TMA-staged kernel; test_gpu_stress.py runs one launch over a
+    surface of more than a wave, and reaches the plain-load kernel from a device source 4 bytes off."""
     lib, oracle = T.product(), T.oracle()
     h, w = 1020, 1028                                        # 255 x 257 = 65535 blocks
     raw = np.random.default_rng(17).integers(0, 256, h * (w + 4) * 4 + 64, dtype=np.uint8)
