@@ -373,6 +373,42 @@ void itw_shard_finalize(void);
 int itw_encode_mip_chain_sharded(int format, const rgba_surface* band0, int width, int height, int levels,
                                  const void* settings, uint8_t* chain, void* cuda_stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Section 8 -- decompress for display and the preview path: what the plug-in's options dialog runs on
+ * every settings change (GetCompressedImageForPreview, IntelPlugin.cpp:933-1080): front end -> encode ->
+ * DirectX::Decompress (DirectXTexCompress.cpp:358-468 -> _ConvertScanline -> _StoreScanline) into the
+ * format the dialog shows.
+ * ------------------------------------------------------------------------------------------- */
+enum {
+    ITW_TARGET_R32G32B32A32_FLOAT = 2,    /* 16 B per texel                                     */
+    ITW_TARGET_R8G8B8A8_UNORM = 28,       /* 4 B per texel                                      */
+    ITW_TARGET_R8G8B8A8_UNORM_SRGB = 29   /* 4 B per texel                                      */
+};
+/* DirectX::Decompress of `blocks` (ceil(width/4) * ceil(height/4) blocks in raster order) into `dst`
+ * (width x height texels of `target_dxgi`; texels of ragged edge blocks outside the image are not written).
+ * Pairs (dxgi_format -> target):
+ *   71/77/83/98 (UNORM)      -> 28: the bytes of itw_decode;  -> 29: XMColorRGBToSRGB, then the UNORM8 store
+ *   80 (BC4 UNORM)           -> 28 / 29: as above with red copied into green and blue, (r, r, r, 255): DirectXTex converts
+ *                               an R format to an RGB one that way (itw_decode gives (r, 0, 0, 255))
+ *   72/78/99 (_SRGB)         -> 28: XMColorSRGBToRGB, then the UNORM8 store;  -> 29: the plain bytes
+ *   95/96 (BC6H UF16 / SF16) -> 28: half -> float -> saturate -> UNORM8;  -> 2: half -> float, alpha 1.0
+ * Other pairs are rejected before anything is enqueued.  Either side may be host or device memory (device
+ * operands: the ordering rule of CompressBlocks*); synchronous.  Returns 0 on success. */
+int itw_decompress(int dxgi_format, const uint8_t* blocks, int width, int height, int target_dxgi,
+                   const rgba_surface* dst);
+/* GetCompressedImageForPreview in one call.  count == 1: a 2-D document; count == 6: six faces of equal size
+ * (+X,-X,+Y,-Y,+Z,-Z) laid out as a 4w x 3h horizontal cross (cells without a face are zero texels, flipped /
+ * normalised like the rest).  Front end (`flags` = ITW_FRONT_*) -> [cross] -> pad -> encode to `dxgi_format`
+ * (`settings` as for itw_encode_device) -> display decompress into `display`, which must have the size of the
+ * image or cross and the texels of the target: R32G32B32A32_FLOAT (16 B) for BC6H at sources[0].depth == 32,
+ * R8G8B8A8_UNORM (4 B) otherwise.  At depth 32 BC1/BC3/BC7 are shown as their _SRGB formats, at depths 8 / 16
+ * _SRGB formats are shown as UNORM (IntelPlugin.cpp:1024-1059).  *compressed_bytes (may be NULL) receives the
+ * size of the encoded image.  Cube maps of BC6H_SF16 are rejected (the plug-in builds that cross as RGBA8).
+ * Everything between the copy-in of the planes and the copy-out of the display stays on the device.  Either
+ * side may be host or device memory; synchronous.  Returns 0 on success. */
+int itw_preview_pixels(int dxgi_format, const itw_pixel_source* sources, int count, uint32_t flags,
+                       const void* settings, const rgba_surface* display, size_t* compressed_bytes);
+
 #ifdef __cplusplus
 }
 #endif

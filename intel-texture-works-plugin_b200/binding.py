@@ -50,7 +50,8 @@ EXPORTS = (["CompressBlocksBC1", "CompressBlocksBC3", "CompressBlocksBC4", "Comp
             "itw_generate_mips_device_f16", "itw_generate_mips_device_srgb", "itw_dds_encode_pixels", "itw_release", "itw_set_devices", "itw_get_devices",
             "itw_begin_deferred", "itw_flush", "GetProcessorCount", "InitWin32Threads", "DestroyThreads", "GetBytesPerBlock",
             "CompressImageMT", "CompressImageST", "CompressImageBC1", "CompressImageBC3",
-            "itw_shard_plan_make", "itw_shard_unique_id", "itw_shard_init", "itw_shard_finalize", "itw_encode_mip_chain_sharded"]
+            "itw_shard_plan_make", "itw_shard_unique_id", "itw_shard_init", "itw_shard_finalize", "itw_encode_mip_chain_sharded",
+            "itw_decompress", "itw_preview_pixels"]
            + ["CompressImageBC7_" + p for p in BC7_PROFILES] + ["CompressImage" + p.replace("bc6h_", "BC6H_") for p in BC6H_PROFILES]
            + ["GetProfile_" + p for p in BC7_PROFILES + BC6H_PROFILES])
 
@@ -272,6 +273,49 @@ class ItwBcn(EncoderApi):
             self.check()
             raise RuntimeError("itw_dds_encode_file failed")
         return out
+
+    def decompress(self, dxgi_format, blocks, width, height, target):
+        """itw_decompress: host blocks -> H x W x 4 image of `target` (uint8 for 28 / 29, float32 for 2)."""
+        blocks = np.ascontiguousarray(np.frombuffer(bytes(blocks), np.uint8))
+        img = np.zeros((height, width, 4), np.float32 if target == 2 else np.uint8)
+        self.decompress_raw(dxgi_format, blocks.ctypes.data, width, height, target, img.ctypes.data, img.strides[0])
+        return img
+
+    def decompress_raw(self, dxgi_format, blocks_ptr, width, height, target, dst_ptr, stride):
+        """itw_decompress on raw addresses (host or device)."""
+        f = self.lib.itw_decompress
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.POINTER(RgbaSurface)]
+        rc = f(dxgi_format, ctypes.c_void_p(blocks_ptr), width, height, target, ctypes.byref(RgbaSurface(dst_ptr, width, height, stride)))
+        self.check()
+        if rc != 0:
+            raise RuntimeError("itw_decompress failed")
+
+    def preview_pixels(self, dxgi_format, faces, flags=0, settings=None):
+        """itw_preview_pixels: `faces` = one or six host numpy H x W x planes arrays -> (display image, compressed bytes).  The
+        display is float32 for BC6H at depth 32, uint8 otherwise; a cube map gives the 4w x 3h cross."""
+        keep = [np.ascontiguousarray(a) for a in faces]
+        h, w = keep[0].shape[:2]
+        if len(keep) == 6:
+            w, h = 4 * w, 3 * h
+        hdr = dxgi_format in (95, 96) and keep[0].itemsize == 4
+        img = np.zeros((h, w, 4), np.float32 if hdr else np.uint8)
+        srcs = (PixelSource * len(keep))(*[PixelSource(a.ctypes.data, a.shape[1], a.shape[0], a.shape[2], a.itemsize * 8, 0) for a in keep])
+        n = self.preview_pixels_raw(dxgi_format, srcs, len(keep), flags, settings, img.ctypes.data, w, h, img.strides[0])
+        return img, n
+
+    def preview_pixels_raw(self, dxgi_format, sources, count, flags, settings, dst_ptr, width, height, stride):
+        f = self.lib.itw_preview_pixels
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.c_int, ctypes.POINTER(PixelSource), ctypes.c_int, ctypes.c_uint32, ctypes.c_void_p,
+                      ctypes.POINTER(RgbaSurface), ctypes.POINTER(ctypes.c_size_t)]
+        sp = ctypes.cast(ctypes.byref(settings), ctypes.c_void_p) if settings is not None else None
+        n = ctypes.c_size_t(0)
+        rc = f(dxgi_format, sources, count, flags, sp, ctypes.byref(RgbaSurface(dst_ptr, width, height, stride)), ctypes.byref(n))
+        self.check()
+        if rc != 0:
+            raise RuntimeError("itw_preview_pixels failed")
+        return n.value
 
     def check(self):
         e = self.last_error()

@@ -53,7 +53,10 @@ struct BitReader {
 // DirectXMath (outside the tree), round-to-nearest is the assumption.  Note that this is NOT bit replication of the 5/6-bit
 // endpoints: 7/31 decodes to 58, not 57.
 ITW_HD u32 unorm8_of(float x) { return (u32)(int)(x * 255.0f + 0.5f); }
-ITW_HD void decode_bc1_colour(u32 (&px)[16], u32 w0, u32 w1, bool force4)
+struct Unorm8Store { ITW_HD static u32 of(float x) { return unorm8_of(x); } };
+// Store::of(float) -> byte is the store applied to DirectXTex's float endpoints / interpolants (display.cuh adds the sRGB ones)
+template <class Store>
+ITW_HD void decode_bc1_colour_as(u32 (&px)[16], u32 w0, u32 w1, bool force4)
 {
     const u32 c0 = w0 & 0xFFFFu, c1 = w0 >> 16;
     const bool four = (c0 > c1) || force4;
@@ -67,10 +70,10 @@ ITW_HD void decode_bc1_colour(u32 (&px)[16], u32 w0, u32 w1, bool force4)
         const float len = f1 - f0;
         const float f2 = four ? (len * (1.0f / 3.0f) + f0) : (len * 0.5f + f0);
         const float f3 = len * (2.0f / 3.0f) + f0;
-        p0 |= unorm8_of(f0) << (8 * c);
-        p1 |= unorm8_of(f1) << (8 * c);
-        p2 |= unorm8_of(f2) << (8 * c);
-        if (four) p3 |= unorm8_of(f3) << (8 * c);
+        p0 |= Store::of(f0) << (8 * c);
+        p1 |= Store::of(f1) << (8 * c);
+        p2 |= Store::of(f2) << (8 * c);
+        if (four) p3 |= Store::of(f3) << (8 * c);
     }
 #pragma unroll
     for (int k = 0; k < 16; k++) {
@@ -78,6 +81,7 @@ ITW_HD void decode_bc1_colour(u32 (&px)[16], u32 w0, u32 w1, bool force4)
         px[k] = (q == 0) ? p0 : ((q == 1) ? p1 : ((q == 2) ? p2 : p3));
     }
 }
+ITW_HD void decode_bc1_colour(u32 (&px)[16], u32 w0, u32 w1, bool force4) { decode_bc1_colour_as<Unorm8Store>(px, w0, w1, force4); }
 // ---- BC3 alpha / BC4 / BC5 channel block -> 16 values ----
 ITW_HD void decode_alpha(u32 (&val)[16], u32 w0, u32 w1)
 {

@@ -25,6 +25,7 @@
 #include "bc4_bc5.cuh"
 #include "mips.cuh"
 #include "decode.cuh"
+#include "display.cuh"
 #include "frontend.cuh"
 #include "mips_f16.cuh"
 #include "itw_params.h"
@@ -1037,3 +1038,4 @@ int itw_bc7_phase_clocks(void* out, size_t bytes)
 #include "itw_dds.inc"
 #include "itw_mips.inc"
 #include "itw_shard.inc"
+#include "itw_preview.inc"
