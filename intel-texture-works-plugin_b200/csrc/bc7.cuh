@@ -13,11 +13,11 @@
 //     and 2, and one walk over both masks' texels searches them for mode 2; then lane <-> (block, shape) adds three stored
 //     mode-2 errors and searches mode 0 from the stored endpoints.  A two-subset shape
 //     (modes 1, 3, 7) belongs to one lane.  When the profile searches all 64 of them for modes 1 / 3, lane <-> (block, shape)
-//     over the four blocks of a group: one routine fits both subsets (bc7_fit_pair: subset 1's moments are the block's minus
-//     subset 0's, two independent PCA lines, one projection loop) and gives the split keys, and one walk over the 16
-//     texels scores modes 1 and 3.  For shorter lists and for mode 7 a lane evaluates one ranked shape: it fits each subset
-//     and searches the shape for both modes of the pair (the pair fit measured slower there: it raises the register
-//     pressure of bc7_eval_shape);
+//     over the four blocks of a group, shapes in popcount order: one routine fits both subsets (bc7_fit_pair: subset 1's
+//     moments are the block's minus subset 0's, two independent PCA lines, one projection loop) and gives the split keys,
+//     and one walk over each subset's texels scores modes 1 and 3.  For shorter lists and for mode 7 a lane evaluates
+//     one ranked shape: it fits each subset and searches the shape for both modes of the pair (the pair fit measured slower
+//     there: it raises the register pressure of bc7_eval_shape);
 //   * ranking phase: lane <-> (block slot, two-subset shape) for the 64 PCA split bounds, only where a list of 0 < t < 64
 //     shapes needs it to choose its members;
 //   * winner phases: lane <-> (block slot, list, strip of 16 entries), then lane <-> (block slot, list);
@@ -51,6 +51,7 @@
 #pragma once
 #include "bc67_core.cuh"
 #include "itw_masks3.cuh"
+#include "itw_order2.cuh"
 
 // unroll factors of the two hottest loops; on H100 (tools/tune_unroll.sh) BC7 slow / basic take 33.65 / 13.51 ms at
 // 16 / 8 against 34.28 / 13.59 (assign 8), 34.81 / 13.85 (assign 4), 33.95 / 13.64 (power 4), 33.90 / 13.60 (power 2)
@@ -66,6 +67,8 @@ namespace itw {
 // distinct subset masks of the three-subset shapes and the mask ids of each shape (tools/gen_mask_tables.py)
 ITW_TABLE_DECL(uint16_t, mask3_unique, ITW_MASK3_COUNT)
 ITW_TABLE_DECL(uint8_t, shape3_mask_id, 64 * 3)
+// the two-subset shapes in ascending popcount of subset 0 (tools/gen_mask_tables.py)
+ITW_TABLE_DECL(uint8_t, shape2_order, 64)
 
 // bc7_enc_settings (ispc_texcomp.h:27-41) flattened to ints for the device
 struct Bc7Params {
@@ -400,7 +403,9 @@ ITW_HD_NOINLINE Bc7Seg bc7_fit(const Bc7Block* blk, int rot, int alpha, u32 mask
 // Both subsets of a two-subset shape of an untransformed block: the same values as bc7_fit of mask0 and of its complement
 // (and, at three channels, their split bounds), with the work the two fits share done once.  Subset 1's integer moments are
 // the block's minus subset 0's (exact); the two lines are independent, so the scheduler can interleave them; one projection
-// loop sends every texel to its own subset's line.
+// loop sends every texel to its own subset's line.  That loop reads the texels from the register planes and selects the line
+// per texel: one set-bit walk per subset with its line in registers (texel words from shared memory, as bc7_pair_error) made
+// the `slow` profile 1.1 % slower on H100.
 struct Bc7Pair { Bc7Seg seg[2]; float bound[2]; };
 template <int CH>
 ITW_HD Bc7Pair bc7_fit_pair_impl(const Bc7Block* blk, u32 mask0)
@@ -504,7 +509,7 @@ ITW_HD_NOINLINE int bc7_split_key(const Bc7Block* blk, int shape, int channels)
 //                                                         except in mode 0 -- reference behaviour, K:1003-1009)
 //   mode 1         one p-bit per pair        K:1024-1052  (a single running error sum over both endpoints)
 //   modes 2,4,5    no p-bit                  K:1054-1065
-ITW_HD_NOINLINE Bc7Packed bc7_quantise(Bc7Seg seg, int mode, int channels)
+ITW_HD Bc7Packed bc7_quantise_impl(const Bc7Seg& seg, int mode, int channels)
 {
     const float (&ep)[8] = seg.v;
     // per-mode constants from nibble tables (mode 0 in the low nibble): nested conditionals on `mode` compile to a jump table
@@ -582,6 +587,14 @@ ITW_HD_NOINLINE Bc7Packed bc7_quantise(Bc7Seg seg, int mode, int channels)
         qq[i] = q;
     }
     return Bc7Packed{dec[0], dec[1], qq[0], qq[1]};
+}
+ITW_HD_NOINLINE Bc7Packed bc7_quantise(Bc7Seg seg, int mode, int channels) { return bc7_quantise_impl(seg, mode, channels); }
+// One three-channel segment for modes 1 and 3 (the full two-subset lists): the same code with the mode and the channel count
+// known at compile time, so that the per-mode constants, the no-p-bit branch and the fourth component fold away.
+struct Bc7Packed13 { Bc7Packed m1, m3; };
+ITW_HD_NOINLINE Bc7Packed13 bc7_quantise13(Bc7Seg seg)
+{
+    return Bc7Packed13{bc7_quantise_impl(seg, 1, 3), bc7_quantise_impl(seg, 3, 3)};
 }
 
 // Index search; K:1133-1193.  ends[2j], ends[2j+1] = decoded endpoints A,B of subset j (RGBA bytes);
@@ -769,30 +782,35 @@ ITW_HD Bc7Err2 bc7_masks_error2(const Bc7Block* blk, u32 mask_a, u32 mask_b, u32
     for (; rb; rb &= rb - 1u) tb += bc7_texel_error2(sb, blk->rgb[popcount32((rb & (0u - rb)) - 1u)]);
     return Bc7Err2{ta, tb};
 }
-// Mode-1 (three-bit) and mode-3 (two-bit) errors of one two-subset shape, mask0 = its subset 0: one walk over the 16 texels,
-// each scored against its own subset's constants.  e1 / e3 = decoded endpoints A, B of subsets 0 and 1 for mode 1 / mode 3.
+// Mode-1 (three-bit) and mode-3 (two-bit) errors of one two-subset shape, mask0 = its subset 0: a walk over subset 0's texels
+// with its constants in registers, then one over subset 1's (the errors are exact integers, so the order of the sums does not
+// matter).  Subset 1's constants are built after the first walk, so that only its four endpoint words are live across it.
+// e1 / e3 = decoded endpoints A, B of subsets 0 and 1 for mode 1 / mode 3.
 struct Bc7PairErr { int mode1, mode3; };
+ITW_HD void bc7_subset_error13(Bc7PairErr& e, const Bc7Block* blk, u32 mask, u32 e1a, u32 e1b, u32 e3a, u32 e3b)
+{
+    const Bc7Sub3 s1 = bc7_sub3(e1a, e1b);
+    const Bc7Sub2 s3 = bc7_sub2(e3a, e3b);
+    const int n = popcount16(mask);
+    u32 rest = mask;
+    // unrolled so that the texel loads of several iterations are in flight at once (as bc7_masks_error2; 4 measured faster
+    // than 2 or 8 on H100, and faster than walking both subsets in one loop)
+#pragma unroll 4
+    for (int i = 0; i < n; i++) {
+        const u32 low = rest & (0u - rest);
+        rest ^= low;
+        const u32 t = blk->rgb[popcount32(low - 1u)];
+        e.mode1 += bc7_texel_error3(s1, t);
+        e.mode3 += bc7_texel_error2(s3, t);
+    }
+}
 ITW_HD_NOINLINE Bc7PairErr bc7_pair_error(const Bc7Block* blk, u32 mask0, u32 e1a0, u32 e1b0, u32 e1a1, u32 e1b1, u32 e3a0,
                                           u32 e3b0, u32 e3a1, u32 e3b1)
 {
-    const Bc7Sub3 m1s0 = bc7_sub3(e1a0, e1b0), m1s1 = bc7_sub3(e1a1, e1b1);
-    const Bc7Sub2 m3s0 = bc7_sub2(e3a0, e3b0), m3s1 = bc7_sub2(e3a1, e3b1);
-    int total1 = 0, total3 = 0;
-    ITW_UNROLL(ITW_BC7_ASSIGN_UNROLL)
-    for (int k = 0; k < 16; k++) {
-        const u32 t = blk->rgb[k];
-        const bool in0 = (mask0 >> k) & 1u;
-        // field by field: a select of whole structs would take their addresses and put both in local memory
-        const Bc7Sub3 s1{in0 ? m1s0.a : m1s1.a, in0 ? m1s0.b : m1s1.b, in0 ? m1s0.cj : m1s1.cj, in0 ? m1s0.fdiv : m1s1.fdiv,
-                         in0 ? m1s0.rdiv : m1s1.rdiv,
-                         Bc7Lerp{in0 ? m1s0.lerp.base_rb : m1s1.lerp.base_rb, in0 ? m1s0.lerp.base_ga : m1s1.lerp.base_ga,
-                                 in0 ? m1s0.lerp.d_rb : m1s1.lerp.d_rb, in0 ? m1s0.lerp.d_ga : m1s1.lerp.d_ga}};
-        const Bc7Sub2 s3{in0 ? m3s0.a : m3s1.a, in0 ? m3s0.b : m3s1.b, in0 ? m3s0.cj : m3s1.cj, in0 ? m3s0.t2 : m3s1.t2,
-                         in0 ? m3s0.t3 : m3s1.t3, in0 ? m3s0.p1 : m3s1.p1, in0 ? m3s0.p2 : m3s1.p2};
-        total1 += bc7_texel_error3(s1, t);
-        total3 += bc7_texel_error2(s3, t);
-    }
-    return Bc7PairErr{total1, total3};
+    Bc7PairErr e{0, 0};
+    bc7_subset_error13(e, blk, mask0, e1a0, e1b0, e3a0, e3b0);
+    bc7_subset_error13(e, blk, ~mask0 & 0xFFFFu, e1a1, e1b1, e3a1, e3b1);
+    return e;
 }
 
 // Least-squares endpoints of one subset from its indices; K:1198-1262.  The sums are exact integers.
@@ -1378,30 +1396,24 @@ ITW_HD void bc7_phase_keys(int lane, Bc7Warp& W, const Bc7Params& P, int g, int 
 // When the longer list holds all 64 shapes (max(t1, t3) = 64: the slow profiles), every shape is fitted and searched anyway
 // and the ranking only decides ties (the winner is the first minimum in ranked order).  Then lane <-> (block, shape) over the
 // whole group: one pair fit (whose first four power iterations give both split bounds, hence the key), quantisation of both
-// subsets for modes 1 and 3, and one walk over the 16 texels for both modes' errors.  Shorter lists (basic: 12 and 8 shapes)
+// subsets for modes 1 and 3 (bc7_quantise13: one call per subset, constants folded), and one walk over each subset's texels
+// for both modes' errors.  Shorter lists (basic: 12 and 8 shapes)
 // rank first and then evaluate only the top t shapes (bc7_phase_keys, bc7_phase_shapes), far fewer fits than all 64.
 ITW_HD bool bc7_full_two(const Bc7Params& P) { return P.sel[1] && maxi(P.t1, P.t3) == 64; }
 ITW_HD void bc7_phase_two_full(int lane, Bc7Warp& W, const Bc7Params& P, int g)
 {
-    for (int t = lane; t < bc7_group_count(W, g) * 64; t += 32) {
-        const int slot = t >> 6, shape = t & 63;
+    const int nv = bc7_group_count(W, g);
+    for (int t = lane; t < nv * 64; t += 32) {
+        // the blocks alternate and the shapes come in popcount order, so that a step holds 8 shapes of similar popcount and
+        // the lanes' subset walks are of similar length; results stay keyed by shape id
+        const int slot = t % nv, shape = ITW_TABLE(shape2_order)[t / nv];
         const Bc7Block* blk = &W.blk[kBc7Slots * g + slot];
         const u32 mask0 = (u32)shape_mask(shape, 0);
         const Bc7Pair f = bc7_fit_pair(blk, mask0, 3);
-        // a list the profile leaves empty walks zero endpoints and is not stored
-        u32 e1[4] = {0u, 0u, 0u, 0u}, e3[4] = {0u, 0u, 0u, 0u};
-#pragma unroll
-        for (int j = 0; j < 2; j++) {
-            if (P.t1 > 0) {
-                const Bc7Packed pk = bc7_quantise(f.seg[j], 1, 3);
-                e1[2 * j] = pk.dec_a; e1[2 * j + 1] = pk.dec_b;
-            }
-            if (P.t3 > 0) {
-                const Bc7Packed pk = bc7_quantise(f.seg[j], 3, 3);
-                e3[2 * j] = pk.dec_a; e3[2 * j + 1] = pk.dec_b;
-            }
-        }
-        const Bc7PairErr e = bc7_pair_error(blk, mask0, e1[0], e1[1], e1[2], e1[3], e3[0], e3[1], e3[2], e3[3]);
+        // both modes are always quantised and scored; a list the profile leaves empty is not stored
+        const Bc7Packed13 q0 = bc7_quantise13(f.seg[0]), q1 = bc7_quantise13(f.seg[1]);
+        const Bc7PairErr e = bc7_pair_error(blk, mask0, q0.m1.dec_a, q0.m1.dec_b, q1.m1.dec_a, q1.m1.dec_b, q0.m3.dec_a,
+                                            q0.m3.dec_b, q1.m3.dec_a, q1.m3.dec_b);
         if (P.t1 > 0) W.cand_err[slot][0][shape] = e.mode1;
         if (P.t3 > 0) W.cand_err[slot][1][shape] = e.mode3;
         W.two.keys[slot][shape] = bc7_key_of(shape, f.bound[0], f.bound[1]);
