@@ -24,8 +24,8 @@
 //   * chain phase: lane <-> (block slot, role).  The per-mode refinement chains, the mode 4/5
 //     rotation / index-swap candidates and mode 6 are independent of one another in the reference
 //     (they only meet in a strict `<` on the final error, K:1358, :1638, :1650, :1684), so they
-//     all run side by side through ONE generic chain routine, and the block's winner is the first
-//     minimum in the reference's order: mode 0, 2, 1, 3, 7, 4(rotation, swap), 5(rotation), 6.
+//     all run side by side through two chain routines, one for the partitioned and one for the one-subset roles, and the
+//     block's winner is the first minimum in the reference's order: mode 0, 2, 1, 3, 7, 4(rotation, swap), 5(rotation), 6.
 //
 // Exactness.  BC7 texels are 8-bit integers, so most of the reference's float arithmetic is exact
 // integer arithmetic in disguise.  Wherever every intermediate is an integer below 2^24 the kernel
@@ -400,6 +400,13 @@ ITW_HD_NOINLINE Bc7Seg bc7_fit(const Bc7Block* blk, int rot, int alpha, u32 mask
     const View v{blk, rot, alpha};
     return (channels == 4) ? bc7_fit_impl<4>(v, mask) : bc7_fit_impl<3>(v, mask);
 }
+// bc7_fit of all sixteen texels (the one-subset chains): the constant mask folds the masking out of the moments and the
+// mask test out of the projection loop; the line and its rounding are bc7_fit's.
+ITW_HD_NOINLINE Bc7Seg bc7_fit_full(const Bc7Block* blk, int rot, int alpha, int channels)
+{
+    const View v{blk, rot, alpha};
+    return (channels == 4) ? bc7_fit_impl<4>(v, 0xFFFFu) : bc7_fit_impl<3>(v, 0xFFFFu);
+}
 // Both subsets of a two-subset shape of an untransformed block: the same values as bc7_fit of mask0 and of its complement
 // (and, at three channels, their split bounds), with the work the two fits share done once.  Subset 1's integer moments are
 // the block's minus subset 0's (exact); the two lines are independent, so the scheduler can interleave them; one projection
@@ -596,13 +603,24 @@ ITW_HD_NOINLINE Bc7Packed13 bc7_quantise13(Bc7Seg seg)
 {
     return Bc7Packed13{bc7_quantise_impl(seg, 1, 3), bc7_quantise_impl(seg, 3, 3)};
 }
+// The same code for one mode and voting channel count known at compile time: the three-subset masks phase (modes 0 and 2)
+// and the one-subset chains (modes 4, 5 and 6), whose passes run one mode in most lanes.
+template <int kMode, int kChannels>
+ITW_HD_NOINLINE Bc7Packed bc7_quantise_m(Bc7Seg seg) { return bc7_quantise_impl(seg, kMode, kChannels); }
+// Modes 4 and 5 have no p-bit, so nothing votes and the channel count does not matter to them.
+ITW_HD Bc7Packed bc7_quantise_one(const Bc7Seg& seg, int mode, int channels)
+{
+    if (mode == 4) return bc7_quantise_m<4, 3>(seg);
+    if (mode == 5) return bc7_quantise_m<5, 3>(seg);
+    return (channels == 4) ? bc7_quantise_m<6, 4>(seg) : bc7_quantise_m<6, 3>(seg);
+}
 
 // Index search; K:1133-1193.  ends[2j], ends[2j+1] = decoded endpoints A,B of subset j (RGBA bytes);
 // chmask zeroes the channels that do not take part (0x00FFFFFF for three-channel modes).
 // Returns the summed error (exact integer) and the sixteen 4-bit indices in idx[0..1].
 // bits_flags = index bits, plus kAssignThresholds when the caller allows the integer-threshold form of the two-bit search.
-// Only the shape phases do: there every lane of the warp searches the same mode at the same time, whereas a chain-phase
-// pass mixes two- and three-bit roles and two texel loops would run one after the other.
+// The shape phases do: there every lane of the warp searches the same mode at the same time.  The partitioned chains do
+// not: their passes pair mode 0 with mode 2 and mode 1 with mode 3, and two texel loops would run one after the other.
 constexpr int kAssignThresholds = 8;
 // Palette, K:1172: ((64 - w) a + w b + 32) >> 6 per channel, two channels per 32-bit word.  Written as (64 a + 32) + w (b - a):
 // the packed difference may borrow across the 16-bit lanes, but every lane of the SUM is the non-negative 14-bit value above,
@@ -668,8 +686,9 @@ ITW_HD Bc7Pick bc7_pick(u32 lo, u32 hi, u32 t)
     return Bc7Pick{first ? e0 : e1, first};
 }
 // bc7_assign's texel loop: palette and per-subset constants from lane-private shared memory.  kThresholds: the two-bit
-// search by thresholds; kIdentity: the texel words are read as stored (every shape-phase search, the partitioned and mode-6
-// chains), else through the rotated view (modes 4 / 5).  Separate instantiations, not a branch inside the loop.
+// search by thresholds; kIdentity: the texel words are read as stored (every shape-phase search and the partitioned
+// chains), else through the rotated view.  Separate instantiations, not a branch inside the loop.  The one-subset chains
+// search with bc7_assign_one.
 template <bool kThresholds, bool kIdentity>
 ITW_HD Bc7Search bc7_assign_texels(const u32 (*pal)[32], int lane, const View& v, int levels, u32 pattern, u32 chmask)
 {
@@ -736,11 +755,14 @@ ITW_HD Bc7Sub2 bc7_sub2(u32 dec_a, u32 dec_b)
     const Bc7Thresholds th = bc7_thresholds(s.idiv);
     return Bc7Sub2{s.a, s.b, s.cj, th.t2, th.t3, s.lerp.entry((u32)bc7_weight(2, 1)), s.lerp.entry((u32)bc7_weight(2, 2))};
 }
+ITW_HD Bc7Pick bc7_pick2(const Bc7Sub2& s, const Bc7Steps& q, u32 t)
+{
+    const u32 lo = q.ge3 ? s.p2 : (q.ge2 ? s.p1 : s.a), hi = q.ge3 ? s.b : (q.ge2 ? s.p2 : s.p1);      // entries q1 - 1, q1
+    return bc7_pick(lo, hi, t);
+}
 ITW_HD int bc7_texel_error2(const Bc7Sub2& s, u32 t)
 {
-    const Bc7Steps q = bc7_steps(bc7_num(t, s.a, s.b, s.cj), s.t2, s.t3);
-    const u32 lo = q.ge3 ? s.p2 : (q.ge2 ? s.p1 : s.a), hi = q.ge3 ? s.b : (q.ge2 ? s.p2 : s.p1);      // entries q1 - 1, q1
-    return bc7_pick(lo, hi, t).err;
+    return bc7_pick2(s, bc7_steps(bc7_num(t, s.a, s.b, s.cj), s.t2, s.t3), t).err;
 }
 // Three-bit constants of one subset
 struct Bc7Sub3 { u32 a, b; int cj; float fdiv, rdiv; Bc7Lerp lerp; };
@@ -754,6 +776,65 @@ ITW_HD int bc7_texel_error3(const Bc7Sub3& s, u32 t)
 {
     const int q1 = bc7_q1_quotient(bc7_num(t, s.a, s.b, s.cj), s.fdiv, s.rdiv, 8.0f, 8);
     return bc7_pick(s.lerp.entry((u32)bc7_weight(3, q1 - 1)), s.lerp.entry((u32)bc7_weight(3, q1)), t).err;
+}
+// Index search of the one-subset chains (modes 4, 5, 6): bc7_assign's texel step with the subset's constants in registers,
+// no subset lookup.  The two-bit searches (mode 4 with index swap 0, mode 5; three channels) take q1 by the thresholds and
+// their two entries from four registers; the three-bit (mode 4 with swap 1) and four-bit (mode 6) searches take the quotient
+// and read the palette from lane-private shared memory.  kIdentity as in bc7_assign_texels.
+ITW_HD void bc7_put_index(u32& out0, u32& out1, int k, int q)
+{
+    const u32 bq = (u32)q << (4 * (k & 7));
+    if (k < 8) out0 += bq; else out1 += bq;
+}
+template <bool kIdentity>
+ITW_HD Bc7Search bc7_assign_one2(const View& v, const Bc7Sub2& s)
+{
+    int total = 0;
+    u32 out0 = 0u, out1 = 0u;
+    ITW_UNROLL(ITW_BC7_ASSIGN_UNROLL)
+    for (int k = 0; k < 16; k++) {
+        const u32 t = kIdentity ? v.b->rgb[k] : (view_tex(v, k) & 0x00FFFFFFu);
+        const Bc7Steps q = bc7_steps(bc7_num(t, s.a, s.b, s.cj), s.t2, s.t3);
+        const Bc7Pick p = bc7_pick2(s, q, t);
+        total += p.err;
+        bc7_put_index(out0, out1, k, p.first ? q.q1() - 1 : q.q1());
+    }
+    return Bc7Search{total, out0, out1};
+}
+template <bool kIdentity>
+ITW_HD Bc7Search bc7_assign_one_quotient(const u32 (*pal)[32], int lane, const View& v, const Bc7Sub& s, int levels, u32 chmask)
+{
+    const u32* tx = (chmask == 0x00FFFFFFu) ? v.b->rgb : v.b->tex;
+    const float fdiv = (float)s.idiv, rdiv = 1.0f / fdiv;           // inf when the endpoints coincide (-> NaN, as 0/0)
+    const float flevels = (float)levels;
+    int total = 0;
+    u32 out0 = 0u, out1 = 0u;
+    ITW_UNROLL(ITW_BC7_ASSIGN_UNROLL)
+    for (int k = 0; k < 16; k++) {
+        const u32 t = kIdentity ? tx[k] : (view_tex(v, k) & chmask);
+        const int q1 = bc7_q1_quotient(bc7_num(t, s.a, s.b, s.cj), fdiv, rdiv, flevels, levels);
+        const Bc7Pick p = bc7_pick(pal[q1 - 1][lane], pal[q1][lane], t);
+        total += p.err;
+        bc7_put_index(out0, out1, k, p.first ? q1 - 1 : q1);
+    }
+    return Bc7Search{total, out0, out1};
+}
+// ea, eb = decoded endpoints A, B; chmask as in bc7_assign (two-bit searches are three-channel)
+ITW_HD_NOINLINE Bc7Search bc7_assign_one(u32 (*pal)[32], int lane, const Bc7Block* blk, int rot, int alpha, int bits, u32 ea,
+                                         u32 eb, u32 chmask)
+{
+    const View v{blk, rot, alpha};
+    if (bits == 2) {
+        const Bc7Sub2 s = bc7_sub2(ea, eb);
+        return (rot == 3) ? bc7_assign_one2<true>(v, s) : bc7_assign_one2<false>(v, s);
+    }
+    const Bc7Sub s = bc7_sub(ea & chmask, eb & chmask);
+    const int levels = 1 << bits;
+    pal[0][lane] = s.a;
+    pal[levels - 1][lane] = s.b;
+    for (int q = 1; q < levels - 1; q++) pal[q][lane] = s.lerp.entry((u32)bc7_weight(bits, q));
+    return (rot == 3) ? bc7_assign_one_quotient<true>(pal, lane, v, s, levels, chmask)
+                      : bc7_assign_one_quotient<false>(pal, lane, v, s, levels, chmask);
 }
 // Mode-2 errors of the two subset masks of a lane pair: a subset's endpoints depend on its mask alone, so the three-subset
 // phases search every distinct mask once.  One counted loop walks the set bits of both masks, so that the two error chains
@@ -1078,85 +1159,78 @@ ITW_HD_NOINLINE Bc7Scalar bc7_scalar_channel(const Bc7Block* blk, int rotation, 
 }
 
 // ---------------------------------------------------------------------------------------------
-// The generic chain: initial fit + refinement + encode of one (block, role); K:1299-1363 (modes
-// 0-3,7), :1565-1655 (modes 4,5), :1657-1689 (mode 6).
+// The chains: initial fit + refinement + encode of one (block, role).  One routine per role kind: the partitioned modes
+// (K:1299-1363: modes 0-3, 7) and the one-subset modes (K:1565-1655: modes 4, 5; K:1657-1689: mode 6).
+// Roles r = 0..4 are the mode slots (modes 0, 2, 1, 3, 7), then mode 4 by (rotation, swap), mode 5 by rotation, mode 6: the
+// reference's order, which decides ties.
 // ---------------------------------------------------------------------------------------------
-struct Role {
-    int kind;      // 0 partitioned, 1 mode 4/5, 2 mode 6
-    int mode, shape, rotation, swap;
-};
 ITW_HD int bc7_rotations(const Bc7Params& P) { return P.sel[2] ? maxi(P.channels - P.ch0, 0) : 0; }
 ITW_HD int bc7_role_count(const Bc7Params& P) { return 5 + 3 * bc7_rotations(P) + (P.sel[3] ? 1 : 0); }
 // The chain phase walks only the roles that can produce a candidate: a partitioned mode whose list is empty under the profile
-// (mode 7 of the RGB profiles, ...) would otherwise idle one lane of every pass.  i-th active role, ascending.
+// (mode 7 of the RGB profiles, ...) would otherwise idle one lane of every pass.
 ITW_HD int bc7_active_roles(const Bc7Params& P)
 {
     int n = bc7_role_count(P) - 5;
     for (int m = 0; m < 5; m++) n += (bc7_slot_count(P, m) > 0) ? 1 : 0;
     return n;
 }
+// i-th active role in RUN order, which groups roles that take the same routine and texel loop, so that the two roles of a
+// sixteen-block pass match: the partitioned modes (0, 2, 1, 3, 7), then the two-bit one-subset searches (mode 4 with swap 0
+// by rotation, mode 5 by rotation), the three-bit ones (mode 4 with swap 1 by rotation) and mode 6.  When the partitioned
+// roles are odd in number, the last of them shares a pass with a one-subset role anyway; mode 6 takes that place, so that
+// the one-subset passes after it stay paired by loop.  The reference's order is the role number r.
 ITW_HD int bc7_active_role(const Bc7Params& P, int i)
 {
+    int nparts = 0;
     for (int m = 0; m < 5; m++)
-        if (bc7_slot_count(P, m) > 0) { if (i == 0) return m; i--; }
-    return 5 + i;
+        if (bc7_slot_count(P, m) > 0) { if (i == 0) return m; i--; nparts++; }
+    const int nrot = bc7_rotations(P), six = 5 + 3 * nrot;
+    if (P.sel[3] && (nparts & 1)) { if (i == 0) return six; i--; }
+    if (i < nrot) return 5 + 2 * i;                              // mode 4, swap 0
+    i -= nrot;
+    if (i < nrot) return 5 + 2 * nrot + i;                       // mode 5
+    i -= nrot;
+    if (i < nrot) return 5 + 2 * i + 1;                          // mode 4, swap 1
+    return six;                                                  // mode 6, when not placed above
+}
+ITW_HD const Bc7Block* bc7_chain_block(const Bc7Warp& W, int slot)
+{
+    return (slot < W.nparked) ? &W.parked[slot] : &W.blk[slot - W.nparked];
 }
 
 struct Bc7Result { int err; u32 code[4]; };
-ITW_HD_NOINLINE Bc7Result bc7_chain(Bc7Warp& W, const Bc7Params& P, int lane, int slot, int r)
+// Partitioned roles r = 0..4: the winning shape of mode slot r, identity view.
+ITW_HD_NOINLINE Bc7Result bc7_chain_parts(Bc7Warp& W, const Bc7Params& P, int lane, int slot, int r)
 {
     Bc7Result res;
     res.err = kErrNone;
     res.code[0] = res.code[1] = res.code[2] = res.code[3] = 0u;
-    const Bc7Block* blk = (slot < W.nparked) ? &W.parked[slot] : &W.blk[slot - W.nparked];
-    const int nrot = bc7_rotations(P);
-    Role role;
-    role.rotation = 3; role.swap = 0; role.shape = 0;
-    if (r < 5) {
-        role.kind = 0;
-        role.mode = bc7_slot_mode(r);
-        role.shape = W.win_shape[slot][r];
-        if (role.shape < 0) return res;
-    } else if (r < 5 + 2 * nrot) {
-        role.kind = 1; role.mode = 4; role.rotation = P.ch0 + ((r - 5) >> 1); role.swap = (r - 5) & 1;
-    } else if (r < 5 + 3 * nrot) {
-        role.kind = 1; role.mode = 5; role.rotation = P.ch0 + (r - 5 - 2 * nrot);
-    } else {
-        role.kind = 2; role.mode = 6;
-    }
-    const int mode = role.mode;
-    const int pairs = bc7_pairs(mode);
-    int bits = bc7_mode_bits(mode);
-    if (role.kind == 1 && role.swap) bits = 3;
+    const int shape = W.win_shape[slot][r];
+    if (shape < 0) return res;
+    const Bc7Block* blk = bc7_chain_block(W, slot);
+    const int mode = bc7_slot_mode(r);
+    const int pairs = bc7_pairs(mode), bits = bc7_mode_bits(mode);
     // channels fitted / searched, and the count that votes on p-bits during refinement (K:1343)
-    const int channels = (role.kind == 2) ? P.channels : ((mode == 7) ? 4 : 3);
-    const int vote_refine = (role.kind == 0) ? P.channels : channels;
+    const int channels = (mode == 7) ? 4 : 3;
     const u32 chmask = (channels == 4) ? 0xFFFFFFFFu : 0x00FFFFFFu;
-    // view: rotation 3 (alpha itself rotated "with itself") is the identity
-    const int rot = (role.kind == 1 && role.rotation < 3) ? role.rotation : 3;
     const int alpha = (P.channels == 4) ? 1 : 0;
-    const u32 pattern = (role.kind == 0) ? shape_pattern(role.shape) : 0u;
+    const u32 pattern = shape_pattern(shape);
 
     u32 ends[6], Q[3][2];
-    // initial candidate
 #pragma unroll
     for (int j = 0; j < 3; j++) {
         Q[j][0] = Q[j][1] = 0u;
         ends[2 * j] = ends[2 * j + 1] = 0u;
     }
-    float tail_a = 0.0f, tail_b = 0.0f;                          // ep[3], ep[7] carried between iterations (quirk Q5)
 #pragma unroll
     for (int j = 0; j < 3; j++) {
         if (j >= pairs) continue;
-        const u32 mask = (role.kind == 0) ? (u32)shape_mask(role.shape, j) : 0xFFFFu;
-        Bc7Seg seg = bc7_fit(blk, rot, alpha, mask, channels);   // slots >= channels are zero (F6)
-        if (role.kind == 2 && channels == 3) seg.v[3] = seg.v[7] = 255.0f;     // K:1664-1667
+        const Bc7Seg seg = bc7_fit(blk, 3, alpha, (u32)shape_mask(shape, j), channels);   // slots >= channels are zero (F6)
         const Bc7Packed pk = bc7_quantise(seg, mode, channels);
-        tail_a = (float)(pk.dec_a >> 24); tail_b = (float)(pk.dec_b >> 24);
         ends[2 * j] = pk.dec_a; ends[2 * j + 1] = pk.dec_b;
         Q[j][0] = pk.q_a; Q[j][1] = pk.q_b;
     }
-    Bc7Search best = bc7_assign(W.palette, lane, blk, rot, alpha, bits, pairs, pattern, ends[0], ends[1], ends[2], ends[3], ends[4],
+    Bc7Search best = bc7_assign(W.palette, lane, blk, 3, alpha, bits, pairs, pattern, ends[0], ends[1], ends[2], ends[3], ends[4],
                                 ends[5], chmask);
 
     const int refine = P.refine[mode];
@@ -1167,47 +1241,83 @@ ITW_HD_NOINLINE Bc7Result bc7_chain(Bc7Warp& W, const Bc7Params& P, int lane, in
 #pragma unroll
         for (int j = 0; j < 3; j++) {
             if (j >= pairs) continue;
-            const u32 mask = (role.kind == 0) ? (u32)shape_mask(role.shape, j) : 0xFFFFu;
-            Bc7Seg seg = bc7_solve(blk, rot, alpha, bits, best.idx0, best.idx1, mask, channels);
-            // K's arrays live across iterations in modes 4-6: a fourth slot the solve does not write keeps the
-            // previous iteration's decoded value
-            if (role.kind != 0 && channels < 4) { seg.v[3] = tail_a; seg.v[7] = tail_b; }
-            const Bc7Packed pk = bc7_quantise(seg, mode, vote_refine);
-            tail_a = (float)(pk.dec_a >> 24); tail_b = (float)(pk.dec_b >> 24);
+            const Bc7Seg seg = bc7_solve(blk, 3, alpha, bits, best.idx0, best.idx1, (u32)shape_mask(shape, j), channels);
+            const Bc7Packed pk = bc7_quantise(seg, mode, P.channels);
             ends[2 * j] = pk.dec_a; ends[2 * j + 1] = pk.dec_b;
             nQ[j][0] = pk.q_a; nQ[j][1] = pk.q_b;
         }
-        const Bc7Search found = bc7_assign(W.palette, lane, blk, rot, alpha, bits, pairs, pattern, ends[0], ends[1], ends[2], ends[3],
+        const Bc7Search found = bc7_assign(W.palette, lane, blk, 3, alpha, bits, pairs, pattern, ends[0], ends[1], ends[2], ends[3],
                                            ends[4], ends[5], chmask);
-        // partitioned modes keep the best iterate (K:1348); modes 4,5,6 keep the last (K:1598-1603, :1677-1682)
-        if (role.kind != 0 || found.err < best.err) {
+        // the best iterate is kept (K:1348)
+        if (found.err < best.err) {
 #pragma unroll
             for (int j = 0; j < 3; j++) { Q[j][0] = nQ[j][0]; Q[j][1] = nQ[j][1]; }
             best = found;
         }
     }
     int best_err = best.err;
-    const u32 best_idx[2] = {best.idx0, best.idx1};
+    if (mode != 7 && P.channels != 3) {                           // opaque error of the dropped alpha; K:1267-1277, :1356
+        int opaque = 0;
+        for (int k = 0; k < 16; k++) { const int d = (int)(blk->tex[k] >> 24) - 255; opaque += d * d; }
+        best_err += opaque;
+    }
+    bc7_write_partitioned(res.code, Q, best.idx0, best.idx1, shape, mode);
+    res.err = best_err;
+    return res;
+}
+// One-subset roles r >= 5: mode 4 (rotation, index swap), mode 5 (rotation), mode 6.  All sixteen texels, the view rotated
+// unless the rotation is 3 (alpha with itself), index search from registers (bc7_assign_one), quantisation with the mode
+// folded (bc7_quantise_one).
+ITW_HD_NOINLINE Bc7Result bc7_chain_one(Bc7Warp& W, const Bc7Params& P, int lane, int slot, int r)
+{
+    Bc7Result res;
+    const Bc7Block* blk = bc7_chain_block(W, slot);
+    const int nrot = bc7_rotations(P);
+    int mode = 6, rotation = 3, swap = 0;
+    if (r < 5 + 2 * nrot) {
+        mode = 4; rotation = P.ch0 + ((r - 5) >> 1); swap = (r - 5) & 1;
+    } else if (r < 5 + 3 * nrot) {
+        mode = 5; rotation = P.ch0 + (r - 5 - 2 * nrot);
+    }
+    const int bits = (mode == 6) ? 4 : ((mode == 4 && swap) ? 3 : 2);
+    const int channels = (mode == 6) ? P.channels : 3;          // fitted, searched and voting (K:1565-1689)
+    const u32 chmask = (channels == 4) ? 0xFFFFFFFFu : 0x00FFFFFFu;
+    const int rot = (rotation < 3) ? rotation : 3;              // rotation 3 (alpha "with itself") is the identity
+    const int alpha = (P.channels == 4) ? 1 : 0;
 
-    u32* out = res.code;
-    if (role.kind == 0) {
-        if (mode != 7 && P.channels != 3) {                       // opaque error of the dropped alpha; K:1267-1277, :1356
-            int opaque = 0;
-            for (int k = 0; k < 16; k++) { const int d = (int)(blk->tex[k] >> 24) - 255; opaque += d * d; }
-            best_err += opaque;
-        }
-        bc7_write_partitioned(out, Q, best_idx[0], best_idx[1], role.shape, mode);
-    } else if (role.kind == 1) {
-        const int abits = (mode == 4 && !role.swap) ? 3 : 2, aepbits = (mode == 4) ? 6 : 8;
-        const Bc7Scalar sc = bc7_scalar_channel(blk, role.rotation, abits, aepbits, P.rch);
+    Bc7Seg seg = bc7_fit_full(blk, rot, alpha, channels);       // slots >= channels are zero (F6)
+    if (mode == 6 && channels == 3) seg.v[3] = seg.v[7] = 255.0f;                // K:1664-1667
+    Bc7Packed pk = bc7_quantise_one(seg, mode, channels);
+    // ep[3], ep[7] are carried between iterations (quirk Q5): a fourth slot the solve does not write keeps the previous
+    // iteration's decoded value
+    float tail_a = (float)(pk.dec_a >> 24), tail_b = (float)(pk.dec_b >> 24);
+    Bc7Search best = bc7_assign_one(W.palette, lane, blk, rot, alpha, bits, pk.dec_a, pk.dec_b, chmask);
+    const int refine = P.refine[mode];
+    for (int it = 0; it < refine; it++) {
+        Bc7Seg s = bc7_solve(blk, rot, alpha, bits, best.idx0, best.idx1, 0xFFFFu, channels);
+        if (channels < 4) { s.v[3] = tail_a; s.v[7] = tail_b; }
+        pk = bc7_quantise_one(s, mode, channels);
+        tail_a = (float)(pk.dec_a >> 24); tail_b = (float)(pk.dec_b >> 24);
+        // the last iterate is kept (K:1598-1603, :1677-1682)
+        best = bc7_assign_one(W.palette, lane, blk, rot, alpha, bits, pk.dec_a, pk.dec_b, chmask);
+    }
+    int best_err = best.err;
+    if (mode != 6) {
+        const int abits = (mode == 4 && !swap) ? 3 : 2, aepbits = (mode == 4) ? 6 : 8;
+        const Bc7Scalar sc = bc7_scalar_channel(blk, rotation, abits, aepbits, P.rch);
         best_err += sc.err;
-        bc7_write_mode45(out, Q[0][0], Q[0][1], best_idx[0], best_idx[1], sc.q0, sc.q1, sc.idx0, sc.idx1, mode, role.rotation,
-                         role.swap);
+        bc7_write_mode45(res.code, pk.q_a, pk.q_b, best.idx0, best.idx1, sc.q0, sc.q1, sc.idx0, sc.idx1, mode, rotation, swap);
     } else {
-        bc7_write_mode6(out, Q[0][0], Q[0][1], best_idx[0], best_idx[1]);
+        bc7_write_mode6(res.code, pk.q_a, pk.q_b, best.idx0, best.idx1);
     }
     res.err = best_err;
     return res;
+}
+
+// One call site in the chain phase: the kernel body around it allocates its registers as for a single callee.
+ITW_HD_NOINLINE Bc7Result bc7_chain(Bc7Warp& W, const Bc7Params& P, int lane, int slot, int r)
+{
+    return (r < 5) ? bc7_chain_parts(W, P, lane, slot, r) : bc7_chain_one(W, P, lane, slot, r);
 }
 
 // =============================================================================================
@@ -1328,13 +1438,13 @@ ITW_HD void bc7_phase_masks3(int lane, Bc7Warp& W, const Bc7Params& P, int g)
         if (ca > 0 && u < ITW_MASK3_FIRST) {                       // ITW_MASK3_FIRST is even: both masks or neither
 #pragma unroll
             for (int j = 0; j < 2; j++) {
-                const Bc7Packed pk = bc7_quantise(f.seg[j], 0, 3);
+                const Bc7Packed pk = bc7_quantise_m<0, 3>(f.seg[j]);
                 W.masks3.ends0[slot][u + j][0] = pk.dec_a;
                 W.masks3.ends0[slot][u + j][1] = pk.dec_b;
             }
         }
         if (cb > 0) {
-            const Bc7Packed pa = bc7_quantise(f.seg[0], 2, 3), pb = bc7_quantise(f.seg[1], 2, 3);
+            const Bc7Packed pa = bc7_quantise_m<2, 3>(f.seg[0]), pb = bc7_quantise_m<2, 3>(f.seg[1]);
             const Bc7Err2 e = bc7_masks_error2(blk, mask_a, mask_b, pa.dec_a, pa.dec_b, pb.dec_a, pb.dec_b);
             W.masks3.err2[slot][u] = e.a;
             W.masks3.err2[slot][u + 1] = e.b;
@@ -1511,8 +1621,10 @@ ITW_HD void bc7_phase_first_min(int lane, Bc7Warp& W, const Bc7Params& P, int g,
 // ITS block in registers.  Sixteen blocks make a pass two roles wide: (mode 0, mode 2), (mode 1, mode 3), (rotation, rotation),
 // ... are equally long, where four-wide passes pair three-subset with two-subset chains and leave the last pass half empty.
 // Fewer blocks (the last round of a launch) run wider passes: with one block, all its roles run in one pass.
-// The first strict minimum in role order is kept (K:1358, :1638, :1650, :1684): a lane meets its roles in ascending order,
-// the store phase compares (error, role).
+// The roles run in bc7_active_role's order, so that the two roles of a pass take the same routine (partitioned or one-subset)
+// and mostly the same texel loop: (mode 0, mode 2), (mode 1, mode 3), then the two-bit mode-4 and mode-5 searches, the
+// three-bit ones and mode 6.  That is not the reference's order, so a lane keeps the minimum of (error, role) and the store
+// phase compares (error, role): the first strict minimum in role order (K:1358, :1638, :1650, :1684).
 ITW_HD void bc7_phase_chains(int lane, Bc7Warp& W, const Bc7Params& P, int nb)
 {
     const int nactive = bc7_active_roles(P);
@@ -1523,7 +1635,7 @@ ITW_HD void bc7_phase_chains(int lane, Bc7Warp& W, const Bc7Params& P, int nb)
         for (int i = lane / nb; i < nactive; i += 32 / nb) {
             const int r = bc7_active_role(P, i);
             const Bc7Result res = bc7_chain(W, P, lane, slot, r);
-            if (res.err < best_err) {
+            if (res.err < best_err || (res.err == best_err && r < best_role)) {
                 best_err = res.err; best_role = r;
 #pragma unroll
                 for (int j = 0; j < 4; j++) code[j] = res.code[j];
