@@ -409,6 +409,47 @@ int itw_decompress(int dxgi_format, const uint8_t* blocks, int width, int height
 int itw_preview_pixels(int dxgi_format, const itw_pixel_source* sources, int count, uint32_t flags,
                        const void* settings, const rgba_surface* display, size_t* compressed_bytes);
 
+/* ---------------------------------------------------------------------------------------------
+ * Section 9 -- the open path: what the plug-in does when it opens a block-compressed DDS file, split as it splits the work:
+ *   DoReadStart    (IntelPlugin.cpp:2419-2612)  LoadFromDDSMemory -> IsAlphaAllOpaque -> layers / planes / depth -> Decompress
+ *                                               to R8G8B8A8_UNORM[_SRGB] or R32G32B32A32_FLOAT
+ *   DoReadContinue (IntelPlugin.cpp:2614-2742)  once per layer: zero a full-size interleaved buffer, copy one image into it
+ * The formats are those of itw_dds_desc: BC1, BC3, BC4, BC5, BC6H UF16 / SF16, BC7 and the _SRGB forms.  BC2, uncompressed and
+ * palettised files are rejected.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct itw_dds_open_info {
+    itw_dds_desc desc;        /* as itw_dds_read_header                                                                */
+    int32_t has_alpha;        /* the plug-in's loadInfo.hasAlpha (:2468-2472): HasAlpha(format) && !IsAlphaAllOpaque() and not
+                                 BC1, where IsAlphaAllOpaque checks every texel of every image (all mips of all items) for a
+                                 decoded alpha below 0.99.  Taken before the cube-map override.                           */
+    int32_t has_mips;         /* mip_levels > 1                                                                         */
+    int32_t ask_user;         /* the plug-in would show its load dialog (:2481-2490, after the cube-map override)        */
+    /* filled by itw_dds_open_layout: */
+    int32_t layers;           /* the number of layers the host creates: 0 (a background image), 1, 6 (a cube map) or
+                                 mip_levels (mips as layers) (:2507-2532)                                               */
+    int32_t calls;            /* itw_dds_read_layer calls = max(1, layers)                                              */
+    int32_t planes, depth;    /* 3 or 4 channels; 8 (bytes) or 32 (floats) bits per channel (:2591-2602)                */
+    int32_t width, height;    /* every layer: the top level (or one cube face)                                          */
+    int32_t target_dxgi;      /* the Decompress target: 28 R8G8B8A8_UNORM, 29 R8G8B8A8_UNORM_SRGB, 2 R32G32B32A32_FLOAT  */
+} itw_dds_open_info;
+/* the load dialog's two answers (:2477-2504), or the values a script supplies */
+enum { ITW_OPEN_SEPARATE_ALPHA = 1, ITW_OPEN_MIPS = 2 };
+/* Header + the alpha check on the GPU.  Fills desc, has_alpha, has_mips and ask_user; zeroes the layout fields.  A file of
+ * array_size 6 (one cube map) is read as a cube map, as the plug-in does.  Returns 0 on success. */
+int itw_dds_open(const uint8_t* file, size_t size, itw_dds_open_info* info);
+/* The layout for the dialog's answers `options` (ITW_OPEN_*); pure arithmetic, no CUDA call.  Cube maps ignore both answers.
+ * Returns 0 on success. */
+int itw_dds_open_layout(itw_dds_open_info* info, uint32_t options);
+/* One DoReadContinue: layer `call` (0 <= call < info->calls) into `dst`, `height` rows of `width` interleaved texels of `planes`
+ * channels of `depth` bits, rows `row_bytes` apart (0 = tightly packed).  Reads cube face `call` (mip 0) of a cube map, mip `call`
+ * of item 0 when mips are layers, the first image otherwise.  Every byte of the layer is written: the image is DirectX::Decompress'ed
+ * (BC4 as (r, r, r, 255), BC6H with alpha 1.0) into the top-left corner, channels 0..planes-1 are copied (BC1's punch-through
+ * alpha included), the rest of the layer is zero, and a cube map with has_alpha gets its last plane set to 255 / 1.0f.  `file` and
+ * `dst` may each be host or device memory (device operands: the ordering rule of CompressBlocks*); synchronous.  Every argument is
+ * checked before anything is enqueued (a truncated file, a file that does not match info->desc, a call out of range, row_bytes
+ * too small, info not laid out): on failure dst is untouched.  Returns 0 on success. */
+int itw_dds_read_layer(const uint8_t* file, size_t size, const itw_dds_open_info* info, int call, void* dst, int64_t row_bytes);
+
 #ifdef __cplusplus
 }
 #endif

@@ -51,7 +51,7 @@ EXPORTS = (["CompressBlocksBC1", "CompressBlocksBC3", "CompressBlocksBC4", "Comp
             "itw_begin_deferred", "itw_flush", "GetProcessorCount", "InitWin32Threads", "DestroyThreads", "GetBytesPerBlock",
             "CompressImageMT", "CompressImageST", "CompressImageBC1", "CompressImageBC3",
             "itw_shard_plan_make", "itw_shard_unique_id", "itw_shard_init", "itw_shard_finalize", "itw_encode_mip_chain_sharded",
-            "itw_decompress", "itw_preview_pixels"]
+            "itw_decompress", "itw_preview_pixels", "itw_dds_open", "itw_dds_open_layout", "itw_dds_read_layer"]
            + ["CompressImageBC7_" + p for p in BC7_PROFILES] + ["CompressImage" + p.replace("bc6h_", "BC6H_") for p in BC6H_PROFILES]
            + ["GetProfile_" + p for p in BC7_PROFILES + BC6H_PROFILES])
 
@@ -67,6 +67,15 @@ FRONT_HAS_ALPHA, FRONT_GAMMA, FRONT_FLIP_X, FRONT_FLIP_Y, FRONT_NORMALIZE = 1, 2
 class DdsDesc(ctypes.Structure):              # include/itw_bcn.h section 3
     _fields_ = [("width", ctypes.c_uint32), ("height", ctypes.c_uint32), ("mip_levels", ctypes.c_uint32),
                 ("array_size", ctypes.c_uint32), ("dxgi_format", ctypes.c_uint32), ("is_cubemap", ctypes.c_uint32)]
+
+
+class DdsOpenInfo(ctypes.Structure):         # include/itw_bcn.h section 9
+    _fields_ = [("desc", DdsDesc), ("has_alpha", ctypes.c_int32), ("has_mips", ctypes.c_int32), ("ask_user", ctypes.c_int32),
+                ("layers", ctypes.c_int32), ("calls", ctypes.c_int32), ("planes", ctypes.c_int32), ("depth", ctypes.c_int32),
+                ("width", ctypes.c_int32), ("height", ctypes.c_int32), ("target_dxgi", ctypes.c_int32)]
+
+
+OPEN_SEPARATE_ALPHA, OPEN_MIPS = 1, 2
 
 
 class ShardPlan(ctypes.Structure):            # include/itw_bcn.h section 7
@@ -316,6 +325,50 @@ class ItwBcn(EncoderApi):
         if rc != 0:
             raise RuntimeError("itw_preview_pixels failed")
         return n.value
+
+    def dds_open(self, file_ptr, size):
+        """itw_dds_open on a raw address (host or device): header + alpha check -> DdsOpenInfo."""
+        f = self.lib.itw_dds_open
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.POINTER(DdsOpenInfo)]
+        info = DdsOpenInfo()
+        rc = f(ctypes.c_void_p(file_ptr), size, ctypes.byref(info))
+        self.check()
+        if rc != 0:
+            raise RuntimeError("itw_dds_open failed")
+        return info
+
+    def dds_open_layout(self, info, options):
+        """itw_dds_open_layout: fills the layout fields of `info` (in place) for the load dialog's answers `options`."""
+        f = self.lib.itw_dds_open_layout
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.POINTER(DdsOpenInfo), ctypes.c_uint32]
+        rc = f(ctypes.byref(info), options)
+        self.check()
+        if rc != 0:
+            raise RuntimeError("itw_dds_open_layout failed")
+        return info
+
+    def dds_read_layer_raw(self, file_ptr, size, info, call, dst_ptr, row_bytes=0):
+        """itw_dds_read_layer on raw addresses (host or device)."""
+        f = self.lib.itw_dds_read_layer
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.POINTER(DdsOpenInfo), ctypes.c_int, ctypes.c_void_p, ctypes.c_int64]
+        rc = f(ctypes.c_void_p(file_ptr), size, ctypes.byref(info), call, ctypes.c_void_p(dst_ptr), row_bytes)
+        self.check()
+        if rc != 0:
+            raise RuntimeError("itw_dds_read_layer failed")
+
+    def dds_open_layers(self, file, options=0):
+        """The plug-in's whole open path on a host DDS blob: (info, [layer arrays of height x width x planes, uint8 or float32])."""
+        file = np.ascontiguousarray(np.frombuffer(bytes(file), np.uint8))
+        info = self.dds_open_layout(self.dds_open(file.ctypes.data, file.size), options)
+        layers = []
+        for call in range(info.calls):
+            out = np.empty((info.height, info.width, info.planes), np.float32 if info.depth == 32 else np.uint8)
+            self.dds_read_layer_raw(file.ctypes.data, file.size, info, call, out.ctypes.data)
+            layers.append(out)
+        return info, layers
 
     def check(self):
         e = self.last_error()

@@ -26,6 +26,7 @@
 #include "mips.cuh"
 #include "decode.cuh"
 #include "display.cuh"
+#include "open.cuh"
 #include "frontend.cuh"
 #include "mips_f16.cuh"
 #include "itw_params.h"
@@ -1039,3 +1040,4 @@ int itw_bc7_phase_clocks(void* out, size_t bytes)
 #include "itw_mips.inc"
 #include "itw_shard.inc"
 #include "itw_preview.inc"
+#include "itw_open.inc"

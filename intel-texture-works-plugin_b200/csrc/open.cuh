@@ -1,0 +1,191 @@
+// open.cuh -- THE OPEN PATH: what the plug-in's DoReadStart / DoReadContinue (IntelPlugin.cpp:2419-2742) do with a block-compressed
+// DDS file, on the GPU.
+//
+//   alpha scan         ScratchImage::IsAlphaAllOpaque (DirectXTexImage.cpp:744-759): _IsAlphaAllOpaqueBC (DirectXTexCompress.cpp:
+//                      472-554) over EVERY image of the file (every mip of every item).  A texel is not opaque when the decoder's
+//                      float alpha is < 0.99f; texels of ragged edge blocks outside the image do not count.  Only BC3 / BC7 (and their
+//                      _SRGB forms) reach it: BC4 / BC5 / BC6H have no alpha, and the plug-in ignores the answer for BC1 (:2469-2471).
+//   layer store        one DoReadContinue: DirectX::Decompress of one image to R8G8B8A8_UNORM[_SRGB] / R32G32B32A32_FLOAT (:2558),
+//                      then the copy of channels 0..planes-1 into the top-left corner of a zeroed, interleaved layer of the top-level
+//                      size (:2646-2727), with the last plane forced to 255 / 1.0f for a cube map with alpha (:2696, :2724).
+//
+// The alpha decision is integer-exact.
+//   BC7: the decoder's float is byte * (1/255) (BC.h:152-155); 252/255 < 0.99f < 253/255, so "not opaque" is byte <= 252.
+//   BC3: D3DXDecodeBC3's alpha palette is a0/255, a1/255, the 7-step interpolants ((8-q)a0 + (q-1)a1) / (7*255), the 5-step ones
+//        ((6-q)a0 + (q-1)a1) / (5*255), 0 and 1.  The interpolant closest to 0.99 below it is 1767/1785 (0.98992) and above it
+//        1768/1785 (0.99048); for 5 steps 1262/1275 and 1263/1275.  Float rounding (a few ulp, ~1e-7) cannot cross 0.99, and
+//        decode_alpha's byte ((N + 3) / 7, (N + 2) / 5) is <= 252 exactly when N <= 1767 (resp. 1262).  So the same byte test holds.
+//   tests/test_dds_open.py checks both against the cut _IsAlphaAllOpaqueBC for every (a0, a1, index) of a BC3 alpha block and every
+//   alpha byte of BC7 modes 5, 6 and 7.
+//
+// open_layer_kernel: a warp covers 32 adjacent 4x4 tiles of one tile row of the LAYER.  Tiles inside the image decode their block with
+// the display decoders (display.cuh) unchanged; the rest of the layer is zeros, so every byte of the layer is written exactly once and
+// no memset pass precedes it.  Each lane packs its tile's row of texels (12, 16, 48 or 64 bytes) into the warp's row in shared memory;
+// the warp then stores that row with 16-byte stores (plus a byte tail at the layer's right edge), so three-plane rows leave as whole
+// 128-byte lines rather than as 12-byte pieces.
+#pragma once
+#include "display.cuh"
+
+namespace itw {
+
+// The first alpha byte that reads as opaque (see above).
+constexpr u32 kOpaqueAlphaMin = 253u;
+
+// One block of an alpha-bearing format (77 BC3, 98 BC7; _SRGB forms decode alike): does a texel inside the image (the first `cols`
+// columns and `rows` rows of the block) have alpha below 0.99?
+template <int kFormat>
+ITW_HD bool open_block_not_opaque(const u32 (&w)[4], int cols, int rows)
+{
+    u32 a[16];
+    if (kFormat == 77) {
+        decode_alpha(a, w[0], w[1]);
+    } else {
+        u32 px[16];
+        decode_bc7(px, w);                 // the reserved mode decodes to alpha 0: not opaque, as in DirectXTex
+#pragma unroll
+        for (int k = 0; k < 16; k++) a[k] = px[k] >> 24;
+    }
+    bool below = false;
+#pragma unroll
+    for (int k = 0; k < 16; k++)
+        if ((k & 3) < cols && (k >> 2) < rows && a[k] < kOpaqueAlphaMin) below = true;
+    return below;
+}
+
+// One image of the alpha scan: its blocks are payload blocks [first, first + bw*bh) (images are stored back to back, item-major,
+// mip-minor, so block index and byte offset agree for the whole payload).
+struct OpenImage {
+    long long first;
+    int bw, width, height;
+};
+
+#if defined(__CUDACC__)
+// One thread per block of every image; `images` sorted by `first`.  *flag becomes 1 if any texel of any image is not opaque.
+template <int kFormat>
+__global__ void __launch_bounds__(256) open_alpha_kernel(const uint8_t* __restrict__ payload, long long nblocks,
+                                                         const OpenImage* __restrict__ images, int nimages, int* __restrict__ flag)
+{
+    const long long id = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    bool below = false;
+    if (id < nblocks) {
+        int lo = 0, hi = nimages - 1;                           // the last image with first <= id
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (images[mid].first <= id) lo = mid;
+            else hi = mid - 1;
+        }
+        const OpenImage im = images[lo];
+        const int local = (int)(id - im.first), by = local / im.bw, bx = local - by * im.bw;
+        u32 w[4];
+        if (kFormat == 77) {                                    // the alpha half of a BC3 block is its first 8 bytes
+            const uint2 v = __ldg(reinterpret_cast<const uint2*>(payload) + 2 * id);
+            w[0] = v.x; w[1] = v.y; w[2] = w[3] = 0u;
+        } else {
+            const uint4 v = __ldg(reinterpret_cast<const uint4*>(payload) + id);
+            w[0] = v.x; w[1] = v.y; w[2] = v.z; w[3] = v.w;
+        }
+        below = open_block_not_opaque<kFormat>(w, min(4, im.width - 4 * bx), min(4, im.height - 4 * by));
+    }
+    if (__any_sync(0xFFFFFFFFu, below) && (threadIdx.x & 31) == 0) *flag = 1;
+}
+
+// One layer: `dst` holds `height` rows of `width` texels of kPlanes channels (bytes for the LDR decoders 71/77/80/83/98, floats for
+// BC6H 95/96), rows `row_bytes` apart; dst and row_bytes are 16-byte aligned.  The image (iw x ih texels, blocks in raster order
+// in `blocks`) lands in the top-left corner.  force_alpha: the last plane of every image texel is 255 / 1.0f.
+template <int kFormat, int kPlanes>
+__global__ void __launch_bounds__(256, 2) open_layer_kernel(const uint8_t* __restrict__ blocks, int iw, int ih, uint8_t* __restrict__ dst,
+                                                         int width, int height, long long row_bytes, bool force_alpha)
+{
+    constexpr bool kHdr = kFormat == 95 || kFormat == 96;
+    constexpr int kTexel = kPlanes * (kHdr ? 4 : 1);            // bytes per layer texel
+    constexpr int kTileRow = 4 * kTexel;                        // bytes of one tile's row: 12, 16, 48 or 64
+    constexpr int kWords = kTileRow / 4;
+    // One layer row of 32 tiles per warp.  Tile rows of 16, 48 and 64 bytes go in as 16-byte stores (lanes 16 and 48 bytes apart
+    // meet 8 distinct bank quads per quarter warp); for 64 bytes one spare 16-byte slot after every 128 bytes (kPad) spreads the
+    // lanes of a quarter warp over all eight quads as well.  12-byte rows go in as words, 3 words apart: no conflict either.
+    constexpr int kVecs = kWords % 4 == 0 ? kWords / 4 : 0;
+    constexpr int kPad = kVecs == 4 ? 1 : 0;
+    constexpr int kSlots = 32 * kTileRow / 16;
+    __shared__ uint4 stage[8][kSlots + kPad * kSlots / 8];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int tw = (width + 3) >> 2, chunks = (tw + 31) >> 5;
+    const long long g = (long long)blockIdx.x * 8 + warp;       // warp-uniform: (tile row, chunk of 32 tiles)
+    if (g >= (long long)((height + 3) >> 2) * chunks) return;
+    const int ty = (int)(g / chunks), chunk = (int)(g - (long long)ty * chunks), tx = 32 * chunk + lane;
+    const int ibw = (iw + 3) >> 2;
+    const bool in_image = tx < ibw && ty < ((ih + 3) >> 2);
+    uint4 v = make_uint4(0u, 0u, 0u, 0u);
+    if (in_image) {
+        const long long id = (long long)ty * ibw + tx;
+        if (kFormat == 71 || kFormat == 80) {
+            const uint2 h = __ldg(reinterpret_cast<const uint2*>(blocks) + id);
+            v.x = h.x; v.y = h.y;
+        } else {
+            v = __ldg(reinterpret_cast<const uint4*>(blocks) + id);
+        }
+    }
+    const u32 w[4] = {v.x, v.y, v.z, v.w};
+    // the tile's texels: four float bit patterns per texel (BC6H) or one RGBA8 word; warps wholly outside the image skip the decode
+    u32 pf[16][4], p8[16];
+    if (__any_sync(0xFFFFFFFFu, in_image)) {
+        if constexpr (kHdr) display_block_f32<kFormat>(pf, w);
+        else display_block_rgba8<kFormat, kDisplayPlain>(p8, w);
+    }
+    const int cols = in_image ? min(4, iw - 4 * tx) : 0;        // texels of this tile that belong to the image
+    const int span = min(128, width - 128 * chunk) * kTexel;    // bytes of the warp's part of a layer row
+    uint8_t* out = dst + (long long)chunk * 128 * kTexel;
+    uint4* srow = stage[warp];
+    auto slot = [](int k) { return k + kPad * (k >> 3); };      // smem slot of the row's k-th 16-byte piece
+#pragma unroll
+    for (int y = 0; y < 4; y++) {
+        const int Y = 4 * ty + y;
+        if (Y >= height) break;
+        const bool row_in = in_image && Y < ih;
+        u32 t[kWords];
+        if constexpr (kHdr) {
+#pragma unroll
+            for (int x = 0; x < 4; x++)
+#pragma unroll
+                for (int c = 0; c < kPlanes; c++) {
+                    u32 v = (row_in && x < cols) ? pf[4 * y + x][c] : 0u;
+                    if (c == kPlanes - 1 && force_alpha && row_in && x < cols) v = 0x3F800000u;
+                    t[kPlanes * x + c] = v;
+                }
+        } else {
+            u32 q[4];
+#pragma unroll
+            for (int x = 0; x < 4; x++) {
+                q[x] = (row_in && x < cols) ? p8[4 * y + x] : 0u;
+                if (force_alpha && row_in && x < cols) q[x] |= 255u << (8 * (kPlanes - 1));
+            }
+            if constexpr (kPlanes == 4) {
+#pragma unroll
+                for (int x = 0; x < 4; x++) t[x] = q[x];
+            } else {                                            // r0 g0 b0 r1 | g1 b1 r2 g2 | b2 r3 g3 b3
+                t[0] = (q[0] & 0x00FFFFFFu) | (q[1] << 24);
+                t[1] = ((q[1] >> 8) & 0xFFFFu) | (q[2] << 16);
+                t[2] = ((q[2] >> 16) & 0xFFu) | (q[3] << 8);
+            }
+        }
+        if (tx < tw) {
+            if constexpr (kVecs > 0) {
+#pragma unroll
+                for (int j = 0; j < kVecs; j++) srow[slot(kVecs * lane + j)] = make_uint4(t[4 * j], t[4 * j + 1], t[4 * j + 2], t[4 * j + 3]);
+            } else {
+                u32* words = reinterpret_cast<u32*>(srow) + lane * kWords;
+#pragma unroll
+                for (int i = 0; i < kWords; i++) words[i] = t[i];
+            }
+        }
+        __syncwarp();
+        uint8_t* grow = out + (long long)Y * row_bytes;
+        const int body = span & ~15;
+        for (int i = lane; i < body >> 4; i += 32) reinterpret_cast<uint4*>(grow)[i] = srow[slot(i)];
+        if (lane < span - body)
+            grow[body + lane] = reinterpret_cast<const uint8_t*>(srow + slot(body >> 4))[lane];
+        __syncwarp();
+    }
+}
+#endif
+
+}  // namespace itw
