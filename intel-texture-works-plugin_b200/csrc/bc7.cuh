@@ -2,9 +2,9 @@
 //
 // Mapping.  One WARP owns kBc7Super = 16 consecutive 4x4 blocks per full round (the last round of a launch deals what is left
 // over every warp of the grid, 1 to 16 blocks each; bc7_kernel).  The shape / ranking phases hold one HALF of eight blocks at
-// a time, as two GROUPS of kBc7Slots = 4 that reuse the per-group scratch; the chain phase -- 14 to 18 roles per block, a
-// quarter of the work -- runs ONCE for all sixteen blocks, two lanes per block, so that a pass is two equally long roles wide
-// (DESIGN.md section 4 has the numbers).
+// a time, as two GROUPS of kBc7Slots = 4 that reuse the per-group scratch; the chain phase -- 14 to 18 roles per block in 8 to
+// 10 units, a third of the work -- runs ONCE for all sixteen blocks, two lanes per block, so that a pass is two equally long
+// units wide (DESIGN.md section 4 has the numbers).
 // The 32 lanes are spread over the blocks' independent work items instead of over texels:
 //   * shape phases: a shape's error is the sum of its subsets' errors, and a subset's fit, endpoints and error depend on its
 //     texel mask alone (the reference refits per shape and mode, K:1279-1297, with identical results).  So the three-subset
@@ -21,11 +21,12 @@
 //   * ranking phase: lane <-> (block slot, two-subset shape) for the 64 PCA split bounds, only where a list of 0 < t < 64
 //     shapes needs it to choose its members;
 //   * winner phases: lane <-> (block slot, list, strip of 16 entries), then lane <-> (block slot, list);
-//   * chain phase: lane <-> (block slot, role).  The per-mode refinement chains, the mode 4/5
+//   * chain phase: lane <-> (block slot, unit of roles).  The per-mode refinement chains, the mode 4/5
 //     rotation / index-swap candidates and mode 6 are independent of one another in the reference
 //     (they only meet in a strict `<` on the final error, K:1358, :1638, :1650, :1684), so they
-//     all run side by side through two chain routines, one for the partitioned and one for the one-subset roles, and the
-//     block's winner is the first minimum in the reference's order: mode 0, 2, 1, 3, 7, 4(rotation, swap), 5(rotation), 6.
+//     all run side by side in units: a partitioned mode, the mode 4/5 roles of one rotation (one fit, one texel walk for
+//     the three searches, the three refinements interleaved), mode 6; the block's winner is the first minimum in the
+//     reference's order: mode 0, 2, 1, 3, 7, 4(rotation, swap), 5(rotation), 6.
 //
 // Exactness.  BC7 texels are 8-bit integers, so most of the reference's float arithmetic is exact
 // integer arithmetic in disguise.  Wherever every intermediate is an integer below 2^24 the kernel
@@ -516,6 +517,12 @@ ITW_HD_NOINLINE int bc7_split_key(const Bc7Block* blk, int shape, int channels)
 //                                                         except in mode 0 -- reference behaviour, K:1003-1009)
 //   mode 1         one p-bit per pair        K:1024-1052  (a single running error sum over both endpoints)
 //   modes 2,4,5    no p-bit                  K:1054-1065
+// decodes four quantised bytes of `bits` bits at once (K:1093-1122): v << (8-d) | that >> d, bytewise
+ITW_HD u32 bc7_decode_packed(u32 q, int bits)
+{
+    const u32 vv = q << (8 - bits);
+    return vv + ((vv >> bits) & (0x01010101u * (0xFFu >> bits)));
+}
 ITW_HD Bc7Packed bc7_quantise_impl(const Bc7Seg& seg, int mode, int channels)
 {
     const float (&ep)[8] = seg.v;
@@ -582,16 +589,11 @@ ITW_HD Bc7Packed bc7_quantise_impl(const Bc7Seg& seg, int mode, int channels)
     }
     if (family == 1) pick1[0] = pick1[1];                                // decided after both endpoints
     if (family == 2) pick1[0] = pick1[1] = false;
-    // decode all four bytes at once (K:1093-1122): v << (8-d) | that >> d, bytewise
-    const int dbits = qbits;                                             // every mode decodes the bits it stores
-    const u32 lowmask = 0x01010101u * (0xFFu >> dbits);
     u32 dec[2], qq[2];
 #pragma unroll
     for (int i = 0; i < 2; i++) {
-        const u32 q = pick1[i] ? cand1[i] : cand0[i];
-        const u32 vv = q << (8 - dbits);
-        dec[i] = vv + ((vv >> dbits) & lowmask);
-        qq[i] = q;
+        qq[i] = pick1[i] ? cand1[i] : cand0[i];
+        dec[i] = bc7_decode_packed(qq[i], qbits);                        // every mode decodes the bits it stores
     }
     return Bc7Packed{dec[0], dec[1], qq[0], qq[1]};
 }
@@ -604,16 +606,10 @@ ITW_HD_NOINLINE Bc7Packed13 bc7_quantise13(Bc7Seg seg)
     return Bc7Packed13{bc7_quantise_impl(seg, 1, 3), bc7_quantise_impl(seg, 3, 3)};
 }
 // The same code for one mode and voting channel count known at compile time: the three-subset masks phase (modes 0 and 2)
-// and the one-subset chains (modes 4, 5 and 6), whose passes run one mode in most lanes.
+// and the mode-6 chain.  The rotation units inline bc7_quantise_impl for modes 4 and 5 (no p-bit, so nothing votes and the
+// channel count does not matter to them).
 template <int kMode, int kChannels>
 ITW_HD_NOINLINE Bc7Packed bc7_quantise_m(Bc7Seg seg) { return bc7_quantise_impl(seg, kMode, kChannels); }
-// Modes 4 and 5 have no p-bit, so nothing votes and the channel count does not matter to them.
-ITW_HD Bc7Packed bc7_quantise_one(const Bc7Seg& seg, int mode, int channels)
-{
-    if (mode == 4) return bc7_quantise_m<4, 3>(seg);
-    if (mode == 5) return bc7_quantise_m<5, 3>(seg);
-    return (channels == 4) ? bc7_quantise_m<6, 4>(seg) : bc7_quantise_m<6, 3>(seg);
-}
 
 // Index search; K:1133-1193.  ends[2j], ends[2j+1] = decoded endpoints A,B of subset j (RGBA bytes);
 // chmask zeroes the channels that do not take part (0x00FFFFFF for three-channel modes).
@@ -688,7 +684,7 @@ ITW_HD Bc7Pick bc7_pick(u32 lo, u32 hi, u32 t)
 // bc7_assign's texel loop: palette and per-subset constants from lane-private shared memory.  kThresholds: the two-bit
 // search by thresholds; kIdentity: the texel words are read as stored (every shape-phase search and the partitioned
 // chains), else through the rotated view.  Separate instantiations, not a branch inside the loop.  The one-subset chains
-// search with bc7_assign_one.
+// search with bc7_assign_rotation and bc7_assign_one.
 template <bool kThresholds, bool kIdentity>
 ITW_HD Bc7Search bc7_assign_texels(const u32 (*pal)[32], int lane, const View& v, int levels, u32 pattern, u32 chmask)
 {
@@ -777,64 +773,64 @@ ITW_HD int bc7_texel_error3(const Bc7Sub3& s, u32 t)
     const int q1 = bc7_q1_quotient(bc7_num(t, s.a, s.b, s.cj), s.fdiv, s.rdiv, 8.0f, 8);
     return bc7_pick(s.lerp.entry((u32)bc7_weight(3, q1 - 1)), s.lerp.entry((u32)bc7_weight(3, q1)), t).err;
 }
-// Index search of the one-subset chains (modes 4, 5, 6): bc7_assign's texel step with the subset's constants in registers,
-// no subset lookup.  The two-bit searches (mode 4 with index swap 0, mode 5; three channels) take q1 by the thresholds and
-// their two entries from four registers; the three-bit (mode 4 with swap 1) and four-bit (mode 6) searches take the quotient
-// and read the palette from lane-private shared memory.  kIdentity as in bc7_assign_texels.
+// Index searches of the one-subset chains: bc7_assign's texel step with the subset's constants in registers, no subset
+// lookup, all sixteen texels.
 ITW_HD void bc7_put_index(u32& out0, u32& out1, int k, int q)
 {
     const u32 bq = (u32)q << (4 * (k & 7));
     if (k < 8) out0 += bq; else out1 += bq;
 }
-template <bool kIdentity>
-ITW_HD Bc7Search bc7_assign_one2(const View& v, const Bc7Sub2& s)
+// Mode 6 (four-bit, identity view): q1 by the quotient, the palette in lane-private shared memory.  ea, eb = decoded
+// endpoints A, B; chmask as in bc7_assign.
+ITW_HD_NOINLINE Bc7Search bc7_assign_one(u32 (*pal)[32], int lane, const Bc7Block* blk, u32 ea, u32 eb, u32 chmask)
 {
-    int total = 0;
-    u32 out0 = 0u, out1 = 0u;
-    ITW_UNROLL(ITW_BC7_ASSIGN_UNROLL)
-    for (int k = 0; k < 16; k++) {
-        const u32 t = kIdentity ? v.b->rgb[k] : (view_tex(v, k) & 0x00FFFFFFu);
-        const Bc7Steps q = bc7_steps(bc7_num(t, s.a, s.b, s.cj), s.t2, s.t3);
-        const Bc7Pick p = bc7_pick2(s, q, t);
-        total += p.err;
-        bc7_put_index(out0, out1, k, p.first ? q.q1() - 1 : q.q1());
-    }
-    return Bc7Search{total, out0, out1};
-}
-template <bool kIdentity>
-ITW_HD Bc7Search bc7_assign_one_quotient(const u32 (*pal)[32], int lane, const View& v, const Bc7Sub& s, int levels, u32 chmask)
-{
-    const u32* tx = (chmask == 0x00FFFFFFu) ? v.b->rgb : v.b->tex;
+    const Bc7Sub s = bc7_sub(ea & chmask, eb & chmask);
+    const int levels = 16;
+    pal[0][lane] = s.a;
+    pal[levels - 1][lane] = s.b;
+    for (int q = 1; q < levels - 1; q++) pal[q][lane] = s.lerp.entry((u32)bc7_weight(4, q));
+    const u32* tx = (chmask == 0x00FFFFFFu) ? blk->rgb : blk->tex;
     const float fdiv = (float)s.idiv, rdiv = 1.0f / fdiv;           // inf when the endpoints coincide (-> NaN, as 0/0)
-    const float flevels = (float)levels;
     int total = 0;
     u32 out0 = 0u, out1 = 0u;
     ITW_UNROLL(ITW_BC7_ASSIGN_UNROLL)
     for (int k = 0; k < 16; k++) {
-        const u32 t = kIdentity ? tx[k] : (view_tex(v, k) & chmask);
-        const int q1 = bc7_q1_quotient(bc7_num(t, s.a, s.b, s.cj), fdiv, rdiv, flevels, levels);
+        const u32 t = tx[k];
+        const int q1 = bc7_q1_quotient(bc7_num(t, s.a, s.b, s.cj), fdiv, rdiv, (float)levels, levels);
         const Bc7Pick p = bc7_pick(pal[q1 - 1][lane], pal[q1][lane], t);
         total += p.err;
         bc7_put_index(out0, out1, k, p.first ? q1 - 1 : q1);
     }
     return Bc7Search{total, out0, out1};
 }
-// ea, eb = decoded endpoints A, B; chmask as in bc7_assign (two-bit searches are three-channel)
-ITW_HD_NOINLINE Bc7Search bc7_assign_one(u32 (*pal)[32], int lane, const Bc7Block* blk, int rot, int alpha, int bits, u32 ea,
-                                         u32 eb, u32 chmask)
+// The three searches of a rotation (bc7_chain_rotation; three channels, rotated view): mode 4 with index swap 0 and mode 5
+// take q1 by the thresholds and their two entries from registers (bc7_pick2), mode 4 with swap 1 takes the three-bit
+// quotient and computes its two entries from the interpolation (bc7_texel_error3).  One walk over the sixteen texels reads
+// each rotated texel once for all three, as bc7_pair_error does for modes 1 and 3.
+struct Bc7Search3 { Bc7Search s[3]; };                // mode 4 swap 0, mode 4 swap 1, mode 5
+ITW_HD Bc7Search3 bc7_assign_rotation(const View& v, u32 a40, u32 b40, u32 a41, u32 b41, u32 a5, u32 b5)
 {
-    const View v{blk, rot, alpha};
-    if (bits == 2) {
-        const Bc7Sub2 s = bc7_sub2(ea, eb);
-        return (rot == 3) ? bc7_assign_one2<true>(v, s) : bc7_assign_one2<false>(v, s);
+    const Bc7Sub2 s40 = bc7_sub2(a40, b40), s5 = bc7_sub2(a5, b5);
+    const Bc7Sub3 s41 = bc7_sub3(a41, b41);
+    Bc7Search3 r;
+#pragma unroll
+    for (int j = 0; j < 3; j++) r.s[j] = Bc7Search{0, 0u, 0u};
+    ITW_UNROLL(ITW_BC7_ASSIGN_UNROLL)
+    for (int k = 0; k < 16; k++) {
+        const u32 t = view_tex(v, k) & 0x00FFFFFFu;
+        const Bc7Steps qa = bc7_steps(bc7_num(t, s40.a, s40.b, s40.cj), s40.t2, s40.t3);
+        const Bc7Steps qc = bc7_steps(bc7_num(t, s5.a, s5.b, s5.cj), s5.t2, s5.t3);
+        const int q1 = bc7_q1_quotient(bc7_num(t, s41.a, s41.b, s41.cj), s41.fdiv, s41.rdiv, 8.0f, 8);
+        const Bc7Pick pa = bc7_pick2(s40, qa, t), pc = bc7_pick2(s5, qc, t);
+        const Bc7Pick pb = bc7_pick(s41.lerp.entry((u32)bc7_weight(3, q1 - 1)), s41.lerp.entry((u32)bc7_weight(3, q1)), t);
+        r.s[0].err += pa.err;
+        r.s[1].err += pb.err;
+        r.s[2].err += pc.err;
+        bc7_put_index(r.s[0].idx0, r.s[0].idx1, k, pa.first ? qa.q1() - 1 : qa.q1());
+        bc7_put_index(r.s[1].idx0, r.s[1].idx1, k, pb.first ? q1 - 1 : q1);
+        bc7_put_index(r.s[2].idx0, r.s[2].idx1, k, pc.first ? qc.q1() - 1 : qc.q1());
     }
-    const Bc7Sub s = bc7_sub(ea & chmask, eb & chmask);
-    const int levels = 1 << bits;
-    pal[0][lane] = s.a;
-    pal[levels - 1][lane] = s.b;
-    for (int q = 1; q < levels - 1; q++) pal[q][lane] = s.lerp.entry((u32)bc7_weight(bits, q));
-    return (rot == 3) ? bc7_assign_one_quotient<true>(pal, lane, v, s, levels, chmask)
-                      : bc7_assign_one_quotient<false>(pal, lane, v, s, levels, chmask);
+    return r;
 }
 // Mode-2 errors of the two subset masks of a lane pair: a subset's endpoints depend on its mask alone, so the three-subset
 // phases search every distinct mask once.  One counted loop walks the set bits of both masks, so that the two error chains
@@ -896,33 +892,18 @@ ITW_HD_NOINLINE Bc7PairErr bc7_pair_error(const Bc7Block* blk, u32 mask0, u32 e1
 
 // Least-squares endpoints of one subset from its indices; K:1198-1262.  The sums are exact integers.
 // Components >= channels are zero.
-ITW_HD_NOINLINE Bc7Seg bc7_solve(const Bc7Block* blk, int rot, int alpha, int bits, u32 idx0, u32 idx1, u32 mask, int channels)
+ITW_HD u32 bc7_index_bytes(u32 idx0, u32 idx1, int i)                     // 4-bit indices of texels 4i..4i+3, one per byte
+{
+    u32 n = (((i < 2) ? idx0 : idx1) >> (16 * (i & 1))) & 0xFFFFu;
+    n = (n | (n << 8)) & 0x00FF00FFu;
+    return (n | (n << 4)) & 0x0F0F0F0Fu;
+}
+// The endpoints from the integer sums: count texels, sq1 = sum q, sqq = sum q^2, sum[c] = sum x_c, atb1[c] = sum (top - q) x_c
+ITW_HD Bc7Seg bc7_solve_ends(u32 top, float count, u32 sq1, u32 sqq, const u32 (&sum)[4], const u32 (&atb1)[4], int channels)
 {
     Bc7Seg seg;
-#pragma unroll
-    for (int i = 0; i < 8; i++) seg.v[i] = 0.0f;
     float (&ep)[8] = seg.v;
-    const View v{blk, rot, alpha};
-    const u32 top = (1u << bits) - 1u;
-    u32 sq1 = 0u, sqq = 0u, sum[4] = {0u, 0u, 0u, 0u}, atb1[4] = {0u, 0u, 0u, 0u};
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-        u32 n = (((i < 2) ? idx0 : idx1) >> (16 * (i & 1))) & 0xFFFFu;     // four 4-bit indices
-        n = (n | (n << 8)) & 0x00FF00FFu;
-        n = (n | (n << 4)) & 0x0F0F0F0Fu;                                  // ... one per byte
-        const u32 bm = nibble_to_bytemask(mask >> (4 * i));
-        const u32 qm = n & bm, ones = bm & 0x01010101u;
-        const u32 xm = ((top * 0x01010101u) & bm) - qm;                    // (levels-1) - q, bytewise, no borrows
-        sq1 = dp4a_u8(qm, 0x01010101u, sq1);
-        sqq = dp4a_u8(qm, qm, sqq);
-#pragma unroll
-        for (int c = 0; c < 4; c++) {                           // channels >= 3; an unused fourth channel sums zeros
-            const u32 p = (c < 3 || channels == 4) ? view_plane(v, c, i) : 0u;
-            sum[c] = dp4a_u8(ones, p, sum[c]);
-            atb1[c] = dp4a_u8(xm, p, atb1[c]);
-        }
-    }
-    const float ftop = (float)top, count = (float)popcount16(mask & 0xFFFFu);
+    const float ftop = (float)top;
     const float fsq1 = (float)sq1, fsqq = (float)sqq;
     float cxx = count * sq(ftop) - (2.0f * ftop) * fsq1 + fsqq;
     float cyy = fsqq;
@@ -945,6 +926,28 @@ ITW_HD_NOINLINE Bc7Seg bc7_solve(const Bc7Block* blk, int rot, int alpha, int bi
         ep[4 + c] = used ? b : 0.0f;
     }
     return seg;
+}
+ITW_HD_NOINLINE Bc7Seg bc7_solve(const Bc7Block* blk, int rot, int alpha, int bits, u32 idx0, u32 idx1, u32 mask, int channels)
+{
+    const View v{blk, rot, alpha};
+    const u32 top = (1u << bits) - 1u;
+    u32 sq1 = 0u, sqq = 0u, sum[4] = {0u, 0u, 0u, 0u}, atb1[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        const u32 n = bc7_index_bytes(idx0, idx1, i);
+        const u32 bm = nibble_to_bytemask(mask >> (4 * i));
+        const u32 qm = n & bm, ones = bm & 0x01010101u;
+        const u32 xm = ((top * 0x01010101u) & bm) - qm;                    // (levels-1) - q, bytewise, no borrows
+        sq1 = dp4a_u8(qm, 0x01010101u, sq1);
+        sqq = dp4a_u8(qm, qm, sqq);
+#pragma unroll
+        for (int c = 0; c < 4; c++) {                           // channels >= 3; an unused fourth channel sums zeros
+            const u32 p = (c < 3 || channels == 4) ? view_plane(v, c, i) : 0u;
+            sum[c] = dp4a_u8(ones, p, sum[c]);
+            atb1[c] = dp4a_u8(xm, p, atb1[c]);
+        }
+    }
+    return bc7_solve_ends(top, (float)popcount16(mask & 0xFFFFu), sq1, sqq, sum, atb1, channels);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1063,42 +1066,55 @@ ITW_HD void scalar_quantise(int (&q)[2], int (&e)[2], const float (&ep)[2], int 
         e[i] = expand_bits(q[i], epbits);
     }
 }
-ITW_HD int scalar_assign(u32& idx0, u32& idx1, const u32 (&pl)[4], int bits, const int (&e)[2])
+// The three scalar channels of a rotation (bc7_chain_rotation), side by side: role r has index bits scalar_bits(r), its
+// endpoints e[r] and gets its indices in idx0[r], idx1[r] and its error in err[r].  One loop reads each plane word once.
+ITW_HD int scalar_bits(int r) { return (r == 0) ? 3 : 2; }            // r = 0, 1, 2: mode 4 swap 0, mode 4 swap 1, mode 5
+ITW_HD int scalar_epbits(int r) { return (r == 2) ? 8 : 6; }
+ITW_HD void scalar_assign3(u32 (&idx0)[3], u32 (&idx1)[3], int (&err)[3], const u32 (&pl)[4], const int (&e)[3][2])
 {
-    const int levels = 1 << bits;
-    const float flevels = (float)levels;
-    const float den = (float)(e[1] - e[0]) + 0.001f, rden = 1.0f / den;
-    unsigned long long pal = 0ull;
+    float den[3], rden[3];
+    unsigned long long pal[3];
+    u32 out[3][2];
 #pragma unroll
-    for (int q = 0; q < 8; q++) {
-        const int w = bc7_weight(bits, q);
-        const u32 v = (q < levels) ? (u32)(((64 - w) * e[0] + w * e[1] + 32) >> 6) : 0u;
-        pal |= (unsigned long long)v << (8 * q);
+    for (int r = 0; r < 3; r++) {
+        const int bits = scalar_bits(r), levels = 1 << bits;
+        den[r] = (float)(e[r][1] - e[r][0]) + 0.001f;
+        rden[r] = 1.0f / den[r];
+        pal[r] = 0ull;
+#pragma unroll
+        for (int q = 0; q < 8; q++) {
+            const int w = bc7_weight(bits, q);
+            const u32 v = (q < levels) ? (u32)(((64 - w) * e[r][0] + w * e[r][1] + 32) >> 6) : 0u;
+            pal[r] |= (unsigned long long)v << (8 * q);
+        }
+        out[r][0] = out[r][1] = 0u;
+        err[r] = 0;
     }
-    u32 out[2] = {0u, 0u};
-    int total = 0;
 #pragma unroll
     for (int h = 0; h < 2; h++) {
 #pragma unroll 1
         for (int i = 0; i < 2; i++) {                          // one plane word = four texels per iteration
-            const u32 word = pl[2 * h + i];
+            const u32 word = i ? pl[2 * h + 1] : pl[2 * h];     // a select: pl[] indexed at run time would be local memory
 #pragma unroll
             for (int j = 0; j < 4; j++) {
                 const int a = (int)((word >> (8 * j)) & 255u);
-                const float proj = div_by_rcp((float)(a - e[0]), den, rden);
-                const int q1 = clampi(trunc_i(fma_rn(proj, flevels, 0.5f)), 1, levels - 1);
-                const u32 two = (u32)(pal >> (8 * (q1 - 1)));  // entries q1-1 and q1
-                const int d0 = (int)(two & 255u) - a, d1 = (int)((two >> 8) & 255u) - a;
-                const int err0 = d0 * d0, err1 = d1 * d1;
-                const bool first = err0 < err1;
-                total += first ? err0 : err1;
-                out[h] += (u32)(first ? q1 - 1 : q1) << (16 * i + 4 * j);
+#pragma unroll
+                for (int r = 0; r < 3; r++) {
+                    const int levels = 1 << scalar_bits(r);
+                    const float proj = div_by_rcp((float)(a - e[r][0]), den[r], rden[r]);
+                    const int q1 = clampi(trunc_i(fma_rn(proj, (float)levels, 0.5f)), 1, levels - 1);
+                    const u32 two = (u32)(pal[r] >> (8 * (q1 - 1)));  // entries q1-1 and q1
+                    const int d0 = (int)(two & 255u) - a, d1 = (int)((two >> 8) & 255u) - a;
+                    const int err0 = d0 * d0, err1 = d1 * d1;
+                    const bool first = err0 < err1;
+                    err[r] += first ? err0 : err1;
+                    out[r][h] += (u32)(first ? q1 - 1 : q1) << (16 * i + 4 * j);
+                }
             }
         }
     }
-    idx0 = out[0];
-    idx1 = out[1];
-    return total;
+#pragma unroll
+    for (int r = 0; r < 3; r++) { idx0[r] = out[r][0]; idx1[r] = out[r][1]; }
 }
 ITW_HD void scalar_solve(float (&ep)[2], const u32 (&pl)[4], int bits, u32 idx0, u32 idx1)
 {
@@ -1129,13 +1145,17 @@ ITW_HD void scalar_solve(float (&ep)[2], const u32 (&pl)[4], int bits, u32 idx0,
         ep[1] = ep[0];
     }
 }
-struct Bc7Scalar { int err, q0, q1; u32 idx0, idx1; };
-ITW_HD_NOINLINE Bc7Scalar bc7_scalar_channel(const Bc7Block* blk, int rotation, int abits, int aepbits, int rch)
+// The scalar channels of mode 4 with swap 0 and 1 and of mode 5 at one rotation: one plane read and one min/max (K:1542-1548)
+// serve all three, the first quantisation of the two mode-4 roles is the same, and the refinements run side by side.  cerr
+// = the errors of the three roles' colour channels; returns the role r (0, 1, 2 as scalar_bits) whose summed error is the
+// first strict minimum, that error and r's scalar channel.
+struct Bc7Scalar { int r, err, q0, q1; u32 idx0, idx1; };
+ITW_HD_NOINLINE Bc7Scalar bc7_scalar_rotation(const Bc7Block* blk, int rotation, int rch, int cerr0, int cerr1, int cerr2)
 {
     u32 pl[4];
 #pragma unroll
     for (int i = 0; i < 4; i++) pl[i] = blk->plane[rotation][i];
-    int lo = 255, hi = 0;                                        // K:1542-1548
+    int lo = 255, hi = 0;
 #pragma unroll
     for (int i = 0; i < 4; i++)
 #pragma unroll
@@ -1144,66 +1164,74 @@ ITW_HD_NOINLINE Bc7Scalar bc7_scalar_channel(const Bc7Block* blk, int rotation, 
             lo = mini(lo, a);
             hi = maxi(hi, a);
         }
-    float ep[2] = {(float)lo, (float)hi};
-    int q[2], e[2];
-    u32 a0, a1;
-    scalar_quantise(q, e, ep, aepbits);
-    int err = scalar_assign(a0, a1, pl, abits, e);
+    float ep[3][2];
+    int q[3][2], e[3][2], err[3];
+    u32 idx0[3], idx1[3];
+    ep[0][0] = (float)lo; ep[0][1] = (float)hi;
+    scalar_quantise(q[0], e[0], ep[0], scalar_epbits(0));
+    scalar_quantise(q[2], e[2], ep[0], scalar_epbits(2));
+#pragma unroll
+    for (int i = 0; i < 2; i++) { q[1][i] = q[0][i]; e[1][i] = e[0][i]; }
+    scalar_assign3(idx0, idx1, err, pl, e);
 #pragma unroll 1
     for (int it = 0; it < rch; it++) {
-        scalar_solve(ep, pl, abits, a0, a1);
-        scalar_quantise(q, e, ep, aepbits);
-        err = scalar_assign(a0, a1, pl, abits, e);
+#pragma unroll
+        for (int r = 0; r < 3; r++) {
+            scalar_solve(ep[r], pl, scalar_bits(r), idx0[r], idx1[r]);
+            scalar_quantise(q[r], e[r], ep[r], scalar_epbits(r));
+        }
+        scalar_assign3(idx0, idx1, err, pl, e);
     }
-    return Bc7Scalar{err, q[0], q[1], a0, a1};
+    const int t0 = cerr0 + err[0], t1 = cerr1 + err[1], t2 = cerr2 + err[2];
+    Bc7Scalar s{0, t0, q[0][0], q[0][1], idx0[0], idx1[0]};
+    if (t1 < s.err) s = Bc7Scalar{1, t1, q[1][0], q[1][1], idx0[1], idx1[1]};
+    if (t2 < s.err) s = Bc7Scalar{2, t2, q[2][0], q[2][1], idx0[2], idx1[2]};
+    return s;
 }
 
 // ---------------------------------------------------------------------------------------------
-// The chains: initial fit + refinement + encode of one (block, role).  One routine per role kind: the partitioned modes
-// (K:1299-1363: modes 0-3, 7) and the one-subset modes (K:1565-1655: modes 4, 5; K:1657-1689: mode 6).
-// Roles r = 0..4 are the mode slots (modes 0, 2, 1, 3, 7), then mode 4 by (rotation, swap), mode 5 by rotation, mode 6: the
-// reference's order, which decides ties.
+// The chains: initial fit + refinement + encode of one (block, role).  Roles r = 0..4 are the mode slots (modes 0, 2, 1, 3,
+// 7), then mode 4 by (rotation, swap), mode 5 by rotation, mode 6: the reference's order, which decides ties.  The chain
+// phase runs them in UNITS, one routine each: a partitioned mode (K:1299-1363: modes 0-3, 7), a rotation (K:1565-1655: the
+// roles of modes 4 and 5 at one rotation) and mode 6 (K:1657-1689).  Units u = 0..4 are the mode slots, then one per
+// rotation, then mode 6.
 // ---------------------------------------------------------------------------------------------
 ITW_HD int bc7_rotations(const Bc7Params& P) { return P.sel[2] ? maxi(P.channels - P.ch0, 0) : 0; }
-ITW_HD int bc7_role_count(const Bc7Params& P) { return 5 + 3 * bc7_rotations(P) + (P.sel[3] ? 1 : 0); }
-// The chain phase walks only the roles that can produce a candidate: a partitioned mode whose list is empty under the profile
+ITW_HD int bc7_unit_count(const Bc7Params& P) { return 5 + bc7_rotations(P) + (P.sel[3] ? 1 : 0); }
+// The chain phase walks only the units that can produce a candidate: a partitioned mode whose list is empty under the profile
 // (mode 7 of the RGB profiles, ...) would otherwise idle one lane of every pass.
-ITW_HD int bc7_active_roles(const Bc7Params& P)
+ITW_HD int bc7_active_units(const Bc7Params& P)
 {
-    int n = bc7_role_count(P) - 5;
+    int n = bc7_unit_count(P) - 5;
     for (int m = 0; m < 5; m++) n += (bc7_slot_count(P, m) > 0) ? 1 : 0;
     return n;
 }
-// i-th active role in RUN order, which groups roles that take the same routine and texel loop, so that the two roles of a
-// sixteen-block pass match: the partitioned modes (0, 2, 1, 3, 7), then the two-bit one-subset searches (mode 4 with swap 0
-// by rotation, mode 5 by rotation), the three-bit ones (mode 4 with swap 1 by rotation) and mode 6.  When the partitioned
-// roles are odd in number, the last of them shares a pass with a one-subset role anyway; mode 6 takes that place, so that
-// the one-subset passes after it stay paired by loop.  The reference's order is the role number r.
-ITW_HD int bc7_active_role(const Bc7Params& P, int i)
+// i-th active unit in RUN order, which groups units that take the same routine, so that the two units of a sixteen-block
+// pass match: the partitioned modes (0, 2, 1, 3, 7), then the rotations and mode 6.  When the partitioned units are odd in
+// number, the last of them shares a pass with a one-subset unit anyway; mode 6 takes that place, so that the rotations
+// after it stay paired.
+ITW_HD int bc7_active_unit(const Bc7Params& P, int i)
 {
     int nparts = 0;
     for (int m = 0; m < 5; m++)
         if (bc7_slot_count(P, m) > 0) { if (i == 0) return m; i--; nparts++; }
-    const int nrot = bc7_rotations(P), six = 5 + 3 * nrot;
+    const int nrot = bc7_rotations(P), six = 5 + nrot;
     if (P.sel[3] && (nparts & 1)) { if (i == 0) return six; i--; }
-    if (i < nrot) return 5 + 2 * i;                              // mode 4, swap 0
-    i -= nrot;
-    if (i < nrot) return 5 + 2 * nrot + i;                       // mode 5
-    i -= nrot;
-    if (i < nrot) return 5 + 2 * i + 1;                          // mode 4, swap 1
-    return six;                                                  // mode 6, when not placed above
+    return (i < nrot) ? 5 + i : six;                             // mode 6, when not placed above
 }
 ITW_HD const Bc7Block* bc7_chain_block(const Bc7Warp& W, int slot)
 {
     return (slot < W.nparked) ? &W.parked[slot] : &W.blk[slot - W.nparked];
 }
 
-struct Bc7Result { int err; u32 code[4]; };
+// the best candidate of a unit: its error, role number and 128 bits
+struct Bc7Result { int err, role; u32 code[4]; };
 // Partitioned roles r = 0..4: the winning shape of mode slot r, identity view.
 ITW_HD_NOINLINE Bc7Result bc7_chain_parts(Bc7Warp& W, const Bc7Params& P, int lane, int slot, int r)
 {
     Bc7Result res;
     res.err = kErrNone;
+    res.role = r;
     res.code[0] = res.code[1] = res.code[2] = res.code[3] = 0u;
     const int shape = W.win_shape[slot][r];
     if (shape < 0) return res;
@@ -1265,59 +1293,149 @@ ITW_HD_NOINLINE Bc7Result bc7_chain_parts(Bc7Warp& W, const Bc7Params& P, int la
     res.err = best_err;
     return res;
 }
-// One-subset roles r >= 5: mode 4 (rotation, index swap), mode 5 (rotation), mode 6.  All sixteen texels, the view rotated
-// unless the rotation is 3 (alpha with itself), index search from registers (bc7_assign_one), quantisation with the mode
-// folded (bc7_quantise_one).
-ITW_HD_NOINLINE Bc7Result bc7_chain_one(Bc7Warp& W, const Bc7Params& P, int lane, int slot, int r)
+// The roles of modes 4 and 5 at one rotation (mode 4 with index swap 0 and 1, mode 5; three channels, all sixteen texels,
+// the view rotated unless the rotation is 3, alpha with itself).  The three share one fit, the two mode-4 roles their first
+// quantisation, and each step of the refinement holds one solve, quantisation and search per role as independent code: the
+// plane sums of the solve are index-free and taken once per step for all three roles (held across the steps they added 4
+// bytes of kernel spills), and one walk over the texels searches all three (bc7_assign_rotation).  Rule F6 and the carried fourth slot (quirk Q5) apply to each role separately.
+// The steps are non-inlined routines that exchange the three roles' state BY VALUE: their quantised endpoints (the decoded
+// ones, and with them the carried fourth slot, follow from those) and their searches.  Nothing else is live across a step,
+// so the chain's call does not raise the registers the chain phase needs around it: with the search as the only call
+// inside the refinement loop, the kernel spilled 112 / 132 bytes instead of 16 / 12 (-Xptxas -v).
+struct Bc7RotState { u32 q[3][2]; Bc7Search3 best; };
+ITW_HD int bc7_rotation_bits(int r) { return (r == 2) ? 7 : 5; }    // stored bits per component, modes 4 and 5
+// the three searches from quantised endpoints
+ITW_HD Bc7Search3 bc7_rotation_search(const View& v, const u32 (&q)[3][2])
 {
-    Bc7Result res;
-    const Bc7Block* blk = bc7_chain_block(W, slot);
-    const int nrot = bc7_rotations(P);
-    int mode = 6, rotation = 3, swap = 0;
-    if (r < 5 + 2 * nrot) {
-        mode = 4; rotation = P.ch0 + ((r - 5) >> 1); swap = (r - 5) & 1;
-    } else if (r < 5 + 3 * nrot) {
-        mode = 5; rotation = P.ch0 + (r - 5 - 2 * nrot);
+    u32 dec[3][2];
+#pragma unroll
+    for (int r = 0; r < 3; r++)
+#pragma unroll
+        for (int i = 0; i < 2; i++) dec[r][i] = bc7_decode_packed(q[r][i], bc7_rotation_bits(r));
+    return bc7_assign_rotation(v, dec[0][0], dec[0][1], dec[1][0], dec[1][1], dec[2][0], dec[2][1]);
+}
+// fit, first quantisations, first searches
+ITW_HD_NOINLINE Bc7RotState bc7_rotation_start(const Bc7Block* blk, int rot, int alpha)
+{
+    const Bc7Seg seg = bc7_fit_full(blk, rot, alpha, 3);        // slots >= 3 are zero (F6)
+    const Bc7Packed p4 = bc7_quantise_impl(seg, 4, 3), p5 = bc7_quantise_impl(seg, 5, 3);
+    Bc7RotState st;
+    st.q[0][0] = st.q[1][0] = p4.q_a; st.q[0][1] = st.q[1][1] = p4.q_b;
+    st.q[2][0] = p5.q_a; st.q[2][1] = p5.q_b;
+    st.best = bc7_rotation_search(View{blk, rot, alpha}, st.q);
+    return st;
+}
+// One refinement step of the roles whose refinement is not over (do4: both mode-4 roles, do5: mode 5); the others keep their
+// state.  s0..s2 = the channel sums of the solve (K:1198-1230), index-free.
+ITW_HD_NOINLINE Bc7RotState bc7_rotation_refine(const Bc7Block* blk, int rot, int alpha, Bc7RotState st, bool do4, bool do5)
+{
+    const View v{blk, rot, alpha};
+    u32 sum[4] = {0u, 0u, 0u, 0u}, sq1[3] = {0u, 0u, 0u}, sqq[3] = {0u, 0u, 0u}, atb1[3][4];
+#pragma unroll
+    for (int r = 0; r < 3; r++) atb1[r][0] = atb1[r][1] = atb1[r][2] = atb1[r][3] = 0u;
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        u32 p[3];
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+            p[c] = view_plane(v, c, i);
+            sum[c] = dp4a_u8(0x01010101u, p[c], sum[c]);
+        }
+#pragma unroll
+        for (int r = 0; r < 3; r++) {
+            const u32 top = (r == 1) ? 7u : 3u;                  // index bits 2, 3, 2
+            const u32 n = bc7_index_bytes(st.best.s[r].idx0, st.best.s[r].idx1, i);
+            const u32 xm = top * 0x01010101u - n;                // (levels-1) - q, bytewise, no borrows
+            sq1[r] = dp4a_u8(n, 0x01010101u, sq1[r]);
+            sqq[r] = dp4a_u8(n, n, sqq[r]);
+#pragma unroll
+            for (int c = 0; c < 3; c++) atb1[r][c] = dp4a_u8(xm, p[c], atb1[r][c]);
+        }
     }
-    const int bits = (mode == 6) ? 4 : ((mode == 4 && swap) ? 3 : 2);
-    const int channels = (mode == 6) ? P.channels : 3;          // fitted, searched and voting (K:1565-1689)
-    const u32 chmask = (channels == 4) ? 0xFFFFFFFFu : 0x00FFFFFFu;
+    Bc7RotState nst;
+#pragma unroll
+    for (int r = 0; r < 3; r++) {
+        Bc7Seg seg = bc7_solve_ends((r == 1) ? 7u : 3u, 16.0f, sq1[r], sqq[r], sum, atb1[r], 3);
+        // ep[3], ep[7] are carried between iterations (quirk Q5): a fourth slot the solve does not write keeps the previous
+        // iteration's decoded value
+        seg.v[3] = (float)(bc7_decode_packed(st.q[r][0], bc7_rotation_bits(r)) >> 24);
+        seg.v[7] = (float)(bc7_decode_packed(st.q[r][1], bc7_rotation_bits(r)) >> 24);
+        const Bc7Packed pk = bc7_quantise_impl(seg, (r == 2) ? 5 : 4, 3);
+        nst.q[r][0] = pk.q_a;
+        nst.q[r][1] = pk.q_b;
+    }
+    nst.best = bc7_rotation_search(v, nst.q);
+    // the last iterate is kept (K:1598-1603)
+#pragma unroll
+    for (int r = 0; r < 3; r++)
+        if (!((r == 2) ? do5 : do4)) { nst.q[r][0] = st.q[r][0]; nst.q[r][1] = st.q[r][1]; nst.best.s[r] = st.best.s[r]; }
+    return nst;
+}
+// The scalar channels (bc7_scalar_rotation), then the 128 bits of the best of the three roles: mode 4 with swap 0 and 1 are
+// roles r4 and r4 + 1, mode 5 is role r5 (r4 < r4 + 1 < r5).
+ITW_HD_NOINLINE Bc7Result bc7_rotation_finish(const Bc7Block* blk, int rotation, int rch, int r4, int r5, Bc7RotState st)
+{
+    const Bc7Scalar sc = bc7_scalar_rotation(blk, rotation, rch, st.best.s[0].err, st.best.s[1].err, st.best.s[2].err);
+    const int w = sc.r;
+    const u32 qa = (w == 0) ? st.q[0][0] : ((w == 1) ? st.q[1][0] : st.q[2][0]);
+    const u32 qb = (w == 0) ? st.q[0][1] : ((w == 1) ? st.q[1][1] : st.q[2][1]);
+    const Bc7Search s = (w == 0) ? st.best.s[0] : ((w == 1) ? st.best.s[1] : st.best.s[2]);
+    Bc7Result res;
+    res.err = sc.err;
+    res.role = (w == 2) ? r5 : r4 + w;
+    bc7_write_mode45(res.code, qa, qb, s.idx0, s.idx1, sc.q0, sc.q1, sc.idx0, sc.idx1, (w == 2) ? 5 : 4, rotation, (w == 1) ? 1 : 0);
+    return res;
+}
+// One rotation (0..3) of a block; n4, n5 = refinement steps of modes 4 and 5, rch = of the scalar channel; roles as in
+// bc7_rotation_finish.  Takes the profile's values by value: a Bc7Params by reference is read from local memory.  Returns
+// the best candidate of the three, the minimum of (error, role).
+ITW_HD_NOINLINE Bc7Result bc7_chain_rotation(const Bc7Block* blk, int rotation, int alpha, int n4, int n5, int rch, int r4, int r5)
+{
     const int rot = (rotation < 3) ? rotation : 3;              // rotation 3 (alpha "with itself") is the identity
+    Bc7RotState st = bc7_rotation_start(blk, rot, alpha);
+#pragma unroll 1
+    for (int it = 0; it < maxi(n4, n5); it++) st = bc7_rotation_refine(blk, rot, alpha, st, it < n4, it < n5);
+    return bc7_rotation_finish(blk, rotation, rch, r4, r5, st);
+}
+// Mode 6 (role 5 + 3 nrot): all sixteen texels and the profile's channels, identity view.
+ITW_HD_NOINLINE Bc7Result bc7_chain_mode6(Bc7Warp& W, const Bc7Params& P, int lane, int slot)
+{
+    const Bc7Block* blk = bc7_chain_block(W, slot);
+    const int channels = P.channels;                            // fitted, searched and voting (K:1657-1689)
+    const u32 chmask = (channels == 4) ? 0xFFFFFFFFu : 0x00FFFFFFu;
     const int alpha = (P.channels == 4) ? 1 : 0;
 
-    Bc7Seg seg = bc7_fit_full(blk, rot, alpha, channels);       // slots >= channels are zero (F6)
-    if (mode == 6 && channels == 3) seg.v[3] = seg.v[7] = 255.0f;                // K:1664-1667
-    Bc7Packed pk = bc7_quantise_one(seg, mode, channels);
-    // ep[3], ep[7] are carried between iterations (quirk Q5): a fourth slot the solve does not write keeps the previous
-    // iteration's decoded value
+    Bc7Seg seg = bc7_fit_full(blk, 3, alpha, channels);         // slots >= channels are zero (F6)
+    if (channels == 3) seg.v[3] = seg.v[7] = 255.0f;            // K:1664-1667
+    Bc7Packed pk = (channels == 4) ? bc7_quantise_m<6, 4>(seg) : bc7_quantise_m<6, 3>(seg);
+    // ep[3], ep[7] are carried between iterations (quirk Q5), as in bc7_chain_rotation
     float tail_a = (float)(pk.dec_a >> 24), tail_b = (float)(pk.dec_b >> 24);
-    Bc7Search best = bc7_assign_one(W.palette, lane, blk, rot, alpha, bits, pk.dec_a, pk.dec_b, chmask);
-    const int refine = P.refine[mode];
+    Bc7Search best = bc7_assign_one(W.palette, lane, blk, pk.dec_a, pk.dec_b, chmask);
+    const int refine = P.refine[6];
     for (int it = 0; it < refine; it++) {
-        Bc7Seg s = bc7_solve(blk, rot, alpha, bits, best.idx0, best.idx1, 0xFFFFu, channels);
+        Bc7Seg s = bc7_solve(blk, 3, alpha, 4, best.idx0, best.idx1, 0xFFFFu, channels);
         if (channels < 4) { s.v[3] = tail_a; s.v[7] = tail_b; }
-        pk = bc7_quantise_one(s, mode, channels);
+        pk = (channels == 4) ? bc7_quantise_m<6, 4>(s) : bc7_quantise_m<6, 3>(s);
         tail_a = (float)(pk.dec_a >> 24); tail_b = (float)(pk.dec_b >> 24);
-        // the last iterate is kept (K:1598-1603, :1677-1682)
-        best = bc7_assign_one(W.palette, lane, blk, rot, alpha, bits, pk.dec_a, pk.dec_b, chmask);
+        // the last iterate is kept (K:1677-1682)
+        best = bc7_assign_one(W.palette, lane, blk, pk.dec_a, pk.dec_b, chmask);
     }
-    int best_err = best.err;
-    if (mode != 6) {
-        const int abits = (mode == 4 && !swap) ? 3 : 2, aepbits = (mode == 4) ? 6 : 8;
-        const Bc7Scalar sc = bc7_scalar_channel(blk, rotation, abits, aepbits, P.rch);
-        best_err += sc.err;
-        bc7_write_mode45(res.code, pk.q_a, pk.q_b, best.idx0, best.idx1, sc.q0, sc.q1, sc.idx0, sc.idx1, mode, rotation, swap);
-    } else {
-        bc7_write_mode6(res.code, pk.q_a, pk.q_b, best.idx0, best.idx1);
-    }
-    res.err = best_err;
+    Bc7Result res;
+    res.err = best.err;
+    res.role = 5 + 3 * bc7_rotations(P);
+    bc7_write_mode6(res.code, pk.q_a, pk.q_b, best.idx0, best.idx1);
     return res;
 }
 
 // One call site in the chain phase: the kernel body around it allocates its registers as for a single callee.
-ITW_HD_NOINLINE Bc7Result bc7_chain(Bc7Warp& W, const Bc7Params& P, int lane, int slot, int r)
+ITW_HD_NOINLINE Bc7Result bc7_chain(Bc7Warp& W, const Bc7Params& P, int lane, int slot, int u)
 {
-    return (r < 5) ? bc7_chain_parts(W, P, lane, slot, r) : bc7_chain_one(W, P, lane, slot, r);
+    if (u < 5) return bc7_chain_parts(W, P, lane, slot, u);
+    const int nrot = bc7_rotations(P), k = u - 5;
+    if (k < nrot)
+        return bc7_chain_rotation(bc7_chain_block(W, slot), P.ch0 + k, (P.channels == 4) ? 1 : 0, P.refine[4], P.refine[5], P.rch,
+                                  5 + 2 * k, 5 + 2 * nrot + k);
+    return bc7_chain_mode6(W, P, lane, slot);
 }
 
 // =============================================================================================
@@ -1615,31 +1733,61 @@ ITW_HD void bc7_phase_first_min(int lane, Bc7Warp& W, const Bc7Params& P, int g,
         W.win_shape[kBc7Batch * W.half + kBc7Slots * g + slot][m] = (best < 0) ? -1 : bc7_slot_shape(W, P, slot, m, best);
     }
 }
+#if defined(__CUDACC__) && defined(ITW_BC7_PHASE_CLOCKS)
+// Per-phase cycle attribution (tools/bc7_phase_clocks.py; not in the product build): thread 0 of every CTA reads clock64()
+// after every barrier and adds the cycles since its previous reading to the phase site it just left.  Sites are numbered in
+// the order the program macros expand them.  In the chain phase of a full round it also times each of its passes as lane 0
+// sees them: divergent lanes are not guaranteed to have reconverged when lane 0 reads the clock, and the atomics sit inside
+// the timed loop, so a pass time is an estimate of the pass, good for comparing passes and builds.
+constexpr int kBc7ClockSites = 40;
+struct Bc7Clocks {
+    unsigned long long site[kBc7ClockSites];     // cycles summed over the CTAs
+    char name[kBc7ClockSites][48];               // the phase call of each site
+    unsigned long long full_sum, full_count;     // cycles of the full rounds (summed) and their number, over the CTAs
+    unsigned long long last_sum, last_max, last_ctas;   // the partial last round: summed, longest CTA, CTAs that ran it
+    unsigned long long pass_sum[kBc7MaxRoles], pass_count[kBc7MaxRoles];   // chain passes of the full rounds
+    int pass_unit[kBc7MaxRoles][2];              // the two units of each such pass (-1: none)
+};
+__device__ Bc7Clocks g_bc7_clocks;
+#endif
 // Chain phase over the whole round.  With nb = per_warp blocks (a power of two, 1..16), lane L works for block L % nb in every
-// pass and runs the active roles L / nb, L / nb + 32 / nb, ...: a pass holds 32 / nb consecutive roles for all blocks, so its
-// lanes run the same KIND of role (partitioned / mode 4-5 / mode 6) almost everywhere, and a lane keeps the best candidate of
-// ITS block in registers.  Sixteen blocks make a pass two roles wide: (mode 0, mode 2), (mode 1, mode 3), (rotation, rotation),
-// ... are equally long, where four-wide passes pair three-subset with two-subset chains and leave the last pass half empty.
-// Fewer blocks (the last round of a launch) run wider passes: with one block, all its roles run in one pass.
-// The roles run in bc7_active_role's order, so that the two roles of a pass take the same routine (partitioned or one-subset)
-// and mostly the same texel loop: (mode 0, mode 2), (mode 1, mode 3), then the two-bit mode-4 and mode-5 searches, the
-// three-bit ones and mode 6.  That is not the reference's order, so a lane keeps the minimum of (error, role) and the store
-// phase compares (error, role): the first strict minimum in role order (K:1358, :1638, :1650, :1684).
+// pass and runs the active units L / nb, L / nb + 32 / nb, ...: a pass holds 32 / nb consecutive units for all blocks, so its
+// lanes run the same KIND of unit (partitioned / rotation / mode 6) almost everywhere, and a lane keeps the best candidate of
+// ITS block in registers.  Sixteen blocks make a pass two units wide: (mode 0, mode 2), (mode 1, mode 3), (rotation,
+// rotation), ... are equally long, where four-wide passes pair three-subset with two-subset chains and leave the last pass
+// half empty.  Fewer blocks (the last round of a launch) run wider passes: with one block, all its units run in one pass.
+// The units run in bc7_active_unit's order, which is not the reference's, so a lane keeps the minimum of (error, role) and
+// the store phase compares (error, role): the first strict minimum in role order (K:1358, :1638, :1650, :1684).
 ITW_HD void bc7_phase_chains(int lane, Bc7Warp& W, const Bc7Params& P, int nb)
 {
-    const int nactive = bc7_active_roles(P);
+    const int nactive = bc7_active_units(P);
     const int slot = lane & (nb - 1);
     int best_err = kErrNone, best_role = 0;
     u32 code[4] = {0u, 0u, 0u, 0u};
+#if defined(__CUDA_ARCH__) && defined(ITW_BC7_PHASE_CLOCKS)
+    const bool timed = threadIdx.x == 0 && nb == kBc7Super;
+    unsigned long long pass_start = clock64();
+#endif
     if (slot < W.ntotal)
         for (int i = lane / nb; i < nactive; i += 32 / nb) {
-            const int r = bc7_active_role(P, i);
-            const Bc7Result res = bc7_chain(W, P, lane, slot, r);
-            if (res.err < best_err || (res.err == best_err && r < best_role)) {
-                best_err = res.err; best_role = r;
+            const int u = bc7_active_unit(P, i);
+            const Bc7Result res = bc7_chain(W, P, lane, slot, u);
+            if (res.err < best_err || (res.err == best_err && res.role < best_role)) {
+                best_err = res.err; best_role = res.role;
 #pragma unroll
                 for (int j = 0; j < 4; j++) code[j] = res.code[j];
             }
+#if defined(__CUDA_ARCH__) && defined(ITW_BC7_PHASE_CLOCKS)
+            if (timed) {
+                const unsigned long long now = clock64();
+                const int p = i / 2;
+                atomicAdd(&g_bc7_clocks.pass_sum[p], now - pass_start);
+                atomicAdd(&g_bc7_clocks.pass_count[p], 1ull);
+                g_bc7_clocks.pass_unit[p][0] = u;
+                g_bc7_clocks.pass_unit[p][1] = (i + 1 < nactive) ? bc7_active_unit(P, i + 1) : -1;
+                pass_start = clock64();
+            }
+#endif
         }
     W.fin.err[lane] = best_err;
     W.fin.role[lane] = best_role;
@@ -1735,17 +1883,6 @@ constexpr int kBc7TileBlocks = kBc7WarpsPerCta * kBc7Super;              // 256
 constexpr int kBc7TileRowBytes = kBc7TileBlocks * 16;                     // 4096
 
 #if defined(ITW_BC7_PHASE_CLOCKS)
-// Per-phase cycle attribution (tools/bc7_phase_clocks.py; not in the product build): thread 0 of every CTA reads clock64()
-// after every barrier and adds the cycles since its previous reading to the phase site it just left.  Sites are numbered in
-// the order the program macros expand them.
-constexpr int kBc7ClockSites = 40;
-struct Bc7Clocks {
-    unsigned long long site[kBc7ClockSites];     // cycles summed over the CTAs
-    char name[kBc7ClockSites][48];               // the phase call of each site
-    unsigned long long full_sum, full_count;     // cycles of the full rounds (summed) and their number, over the CTAs
-    unsigned long long last_sum, last_max, last_ctas;   // the partial last round: summed, longest CTA, CTAs that ran it
-};
-__device__ Bc7Clocks g_bc7_clocks;
 __device__ void bc7_clock_tick(int site, const char* name, unsigned long long& last)
 {
     const unsigned long long now = clock64();

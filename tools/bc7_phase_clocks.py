@@ -2,7 +2,8 @@
 
 Builds the library with -DITW_BC7_PHASE_CLOCKS (thread 0 of every CTA reads clock64() after every barrier of the kernel and
 adds the cycles since its previous reading to that phase site) to a separate path, encodes device-resident surfaces, and
-prints each site's share of the summed CTA cycles, the mean cycles of a full round and those of the last round.
+prints each site's share of the summed CTA cycles, the mean cycles of a full round and those of the last round, and the
+cycles of each pass of the chain phase with the two units it ran.
 
     python tools/bc7_phase_clocks.py                      # slow and basic at 4096 x 4096
     python tools/bc7_phase_clocks.py --build-only --out /tmp/clocks/libitw_bcn.so
@@ -20,12 +21,25 @@ ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
 sys.path.insert(0, ROOT)
 PKG = "intel-texture-works-plugin_b200"
 SITES = 40                                                  # kBc7ClockSites
+MAX_ROLES = 18                                              # kBc7MaxRoles
 
 
 class Bc7Clocks(ctypes.Structure):                           # csrc/bc7.cuh
     _fields_ = [("site", ctypes.c_uint64 * SITES), ("name", (ctypes.c_char * 48) * SITES),
                 ("full_sum", ctypes.c_uint64), ("full_count", ctypes.c_uint64),
-                ("last_sum", ctypes.c_uint64), ("last_max", ctypes.c_uint64), ("last_ctas", ctypes.c_uint64)]
+                ("last_sum", ctypes.c_uint64), ("last_max", ctypes.c_uint64), ("last_ctas", ctypes.c_uint64),
+                ("pass_sum", ctypes.c_uint64 * MAX_ROLES), ("pass_count", ctypes.c_uint64 * MAX_ROLES),
+                ("pass_unit", (ctypes.c_int * 2) * MAX_ROLES)]
+
+
+def unit_name(s, u):
+    """Label of chain unit u under settings s (bc7_chain's numbering): a mode slot, a rotation of modes 4/5 or mode 6."""
+    if u < 0:
+        return "-"
+    if u < 5:
+        return "m" + "02137"[u]
+    nrot = max(s.channels - s.mode45_channel0, 0) if s.mode_selection[2] else 0
+    return f"R{s.mode45_channel0 + u - 5}" if u < 5 + nrot else "m6"
 
 
 def build(out):
@@ -82,6 +96,15 @@ def measure(lib_path, profiles, size, steps):
                   f"last round: {c.last_ctas // steps} CTAs per encode, longest {c.last_max:,} cycles")
         else:
             print("last round: none (the surface is a whole number of full rounds)")
+        chain = sum(c.pass_sum)
+        if chain:
+            print("chain passes of the full rounds (lane 0 of warp 0 of each CTA):")
+            print(f"{'pass':>4}  {'units':<12}  {'of chain':>8}  {'of all':>7}  {'cycles/pass':>11}")
+            for p in range(MAX_ROLES):
+                if c.pass_count[p]:
+                    units = ", ".join(unit_name(settings, u) for u in c.pass_unit[p] if u >= 0)
+                    print(f"{p:>4}  {units:<12}  {100.0 * c.pass_sum[p] / chain:7.2f}%  "
+                          f"{100.0 * c.pass_sum[p] / total:6.2f}%  {c.pass_sum[p] / c.pass_count[p]:11,.0f}")
 
 
 def main():
