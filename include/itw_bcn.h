@@ -333,6 +333,32 @@ int itw_encode_pixels(int format, const itw_pixel_source* src, uint32_t flags, c
 size_t itw_dds_encode_pixels(const itw_dds_desc* desc, const itw_pixel_source* sources, uint32_t flags,
                              const void* settings, uint8_t* file, size_t capacity);
 
+/* The save dialog's "mip maps from layers" option (DoWriteDDS, IntelPlugin.cpp:2093-2145 -> CopyLayersIntoMipMaps,
+ * :1749-1850): each document layer supplies one mip level by hand.  Level l is read from the top-left
+ * max(1, W >> l) x max(1, H >> l) texels of layer l, one planar buffer per channel, as ReadLayerData delivers them. */
+typedef struct itw_layer_source {  /* one document layer as CopyLayersIntoMipMaps reads it                      */
+    const void* channels[3];       /* compositeChannelsList in order: planar, the composite's depth, document-sized */
+    int32_t channel_count;         /* 1..3                                                                       */
+    const void* alpha;             /* layerMask, else transparency; NULL = FillLayerDataToWhite                   */
+    int64_t row_bytes;             /* bytes between rows of every plane; 0 = width * depth / 8                   */
+} itw_layer_source;
+/* itw_dds_encode_pixels for a 2-D texture (array_size 1, not a cube map) whose levels come from `layers`, in the
+ * plug-in's order: convert the composite -> layer 0 overwrites level 0 -> FlipXYChannelNormalMap on level 0 -> mip
+ * chain from level 0 -> layer l overwrites level l for 1 <= l < min(layer_count, mip_levels) (extra layers are
+ * ignored; levels without a layer keep the generated texels) -> NormalizeNormalMapChain on every level -> pad ->
+ * encode.  So levels 1 and up taken from layers are NOT flipped, and generated levels come from the flipped level 0.
+ * Per texel (CopyFromLayerChannelIntoImage, :1694-1741): channel c goes to plane c with the composite's converters,
+ * except that RGBA8 targets at depth 32 always take the v^(1/2.2) step (ITW_FRONT_GAMMA does not matter here);
+ * planes c >= channel_count keep what they held.  Plane 3 is ALWAYS written: from `alpha` when ITW_FRONT_HAS_ALPHA
+ * is set and `alpha` is not NULL, else from white (FillLayerDataToWhite, :1664-1689).  At depth 16 that white is
+ * ConvertTo16Bit((unsigned8)255) = 15360, not 32768, so a level from a 16-bit layer without alpha has alpha 119
+ * (RGBA8) or 0x3780 (RGBA16F) where the composite gives 255 / 0x3C00 -- the plug-in's behaviour, reproduced.
+ * `flags` and `settings` as for itw_dds_encode_pixels; layer_count == 0 gives that function's file.  Every operand
+ * may be in host or device memory; only the read rectangles are copied.  Synchronous.  Returns the file size, or 0
+ * with an error text and `file` untouched when an argument is wrong (nothing is enqueued then). */
+size_t itw_dds_encode_layers(const itw_dds_desc* desc, const itw_pixel_source* composite, const itw_layer_source* layers,
+                             int layer_count, uint32_t flags, const void* settings, uint8_t* file, size_t capacity);
+
 /* ---------------------------------------------------------------------------------------------
  * Section 7 -- row-sharded encode over several GPUs, one process per GPU (SURVEY.md 8e, config C4):
  * "images shard row-wise across the GPUs with a single NCCL all-gather of the packed output".

@@ -51,7 +51,8 @@ EXPORTS = (["CompressBlocksBC1", "CompressBlocksBC3", "CompressBlocksBC4", "Comp
             "itw_begin_deferred", "itw_flush", "GetProcessorCount", "InitWin32Threads", "DestroyThreads", "GetBytesPerBlock",
             "CompressImageMT", "CompressImageST", "CompressImageBC1", "CompressImageBC3",
             "itw_shard_plan_make", "itw_shard_unique_id", "itw_shard_init", "itw_shard_finalize", "itw_encode_mip_chain_sharded",
-            "itw_decompress", "itw_preview_pixels", "itw_dds_open", "itw_dds_open_layout", "itw_dds_read_layer"]
+            "itw_decompress", "itw_preview_pixels", "itw_dds_open", "itw_dds_open_layout", "itw_dds_read_layer",
+            "itw_dds_encode_layers"]
            + ["CompressImageBC7_" + p for p in BC7_PROFILES] + ["CompressImage" + p.replace("bc6h_", "BC6H_") for p in BC6H_PROFILES]
            + ["GetProfile_" + p for p in BC7_PROFILES + BC6H_PROFILES])
 
@@ -59,6 +60,11 @@ EXPORTS = (["CompressBlocksBC1", "CompressBlocksBC3", "CompressBlocksBC4", "Comp
 class PixelSource(ctypes.Structure):          # include/itw_bcn.h section 6
     _fields_ = [("data", ctypes.c_void_p), ("width", ctypes.c_int32), ("height", ctypes.c_int32), ("planes", ctypes.c_int32),
                 ("depth", ctypes.c_int32), ("row_bytes", ctypes.c_int64)]
+
+
+class LayerSource(ctypes.Structure):          # include/itw_bcn.h section 6
+    _fields_ = [("channels", ctypes.c_void_p * 3), ("channel_count", ctypes.c_int32), ("alpha", ctypes.c_void_p),
+                ("row_bytes", ctypes.c_int64)]
 
 
 FRONT_HAS_ALPHA, FRONT_GAMMA, FRONT_FLIP_X, FRONT_FLIP_Y, FRONT_NORMALIZE = 1, 2, 4, 8, 16
@@ -268,6 +274,41 @@ class ItwBcn(EncoderApi):
             self.check()
             raise RuntimeError("itw_dds_encode_pixels failed")
         return out
+
+    def dds_encode_layers(self, desc, composite, layers, flags=0, settings=None):
+        """itw_dds_encode_layers: `composite` = host numpy H x W x planes array; `layers` = one entry per document layer, each a
+        (channels, alpha) pair: 1..3 H x W numpy planes of the composite's dtype, and an H x W plane or None (white)."""
+        n = self.lib.itw_dds_file_bytes(ctypes.byref(desc))
+        if not n:
+            raise ValueError("unsupported DDS description")
+        comp = np.ascontiguousarray(composite)
+        keep = []
+        srcs = (LayerSource * max(1, len(layers)))()
+        for i, (channels, alpha) in enumerate(layers):
+            planes = [np.ascontiguousarray(c, comp.dtype) for c in channels]
+            a = None if alpha is None else np.ascontiguousarray(alpha, comp.dtype)
+            keep += planes + [a]
+            srcs[i].channel_count = len(planes)
+            for c, pl in enumerate(planes):
+                srcs[i].channels[c] = pl.ctypes.data
+            srcs[i].alpha = None if a is None else a.ctypes.data
+            srcs[i].row_bytes = 0
+        src = PixelSource(comp.ctypes.data, comp.shape[1], comp.shape[0], comp.shape[2], comp.itemsize * 8, 0)
+        out = np.zeros(n, np.uint8)
+        sp = ctypes.cast(ctypes.byref(settings), ctypes.c_void_p) if settings is not None else None
+        got = self.dds_encode_layers_raw(desc, src, srcs, len(layers), flags, sp, out.ctypes.data, n)
+        if got != n:
+            self.check()
+            raise RuntimeError("itw_dds_encode_layers failed: " + self.last_error())
+        return out
+
+    def dds_encode_layers_raw(self, desc, composite, layers, count, flags, settings_ptr, file_ptr, capacity):
+        """itw_dds_encode_layers on ctypes structures and raw addresses; returns the file size (0 on error)."""
+        f = self.lib.itw_dds_encode_layers
+        f.restype = ctypes.c_size_t
+        f.argtypes = [ctypes.POINTER(DdsDesc), ctypes.POINTER(PixelSource), ctypes.POINTER(LayerSource), ctypes.c_int, ctypes.c_uint32,
+                      ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t]
+        return f(ctypes.byref(desc), ctypes.byref(composite), layers, count, flags, settings_ptr, file_ptr, capacity)
 
     def dds_encode_file(self, desc, images, settings=None):
         """itw_dds_encode_file: `images` = host numpy arrays, item-major / mip-minor, padded to multiples of 4."""

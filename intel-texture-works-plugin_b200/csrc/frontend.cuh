@@ -134,6 +134,21 @@ ITW_HD void front_normalize_hdr(u32& r, u32& g, u32& b)
     } else { r = 0u; g = 0u; b = 0x3C00u; }
 }
 
+// FlipXYChannelNormalMap on one texel: IP:1519-1527 (bytes) and IP:1531-1542 (halves)
+ITW_HD void front_flip_ldr(u32& r, u32& g, u32 flags)
+{
+    if (flags & kFrontFlipX) r = 255u - r;
+    if (flags & kFrontFlipY) g = 255u - g;
+}
+ITW_HD void front_flip_hdr(u32& r, u32& g, u32 flags)
+{
+    if (flags & (kFrontFlipX | kFrontFlipY)) {
+        const float fr = front_float_from_half(r), fg = front_float_from_half(g);
+        if (flags & kFrontFlipX) r = front_half_from_float(1.0f - fr);
+        if (flags & kFrontFlipY) g = front_half_from_float(1.0f - fg);
+    }
+}
+
 // raw[c] = element of plane c (valid for c < planes) -> out[0] (RGBA8) or out[0..1] (RGBA16F: r | g << 16, b | a << 16)
 ITW_HD void front_compose(u32 (&out)[2], const FrontParams& P, const u32 (&raw)[4])
 {
@@ -144,11 +159,7 @@ ITW_HD void front_compose(u32 (&out)[2], const FrontParams& P, const u32 (&raw)[
         u32 g = (P.planes > 1) ? front_hdr_value(raw[1], P.depth) : 0u;
         u32 b = (P.planes > 2) ? front_hdr_value(raw[2], P.depth) : 0u;
         const u32 a = alpha ? front_hdr_value((P.depth == 32) ? raw[2] : raw[3], P.depth) : 0x3C00u;
-        if (P.flags & (kFrontFlipX | kFrontFlipY)) {                                              // IP:1531-1542
-            const float fr = front_float_from_half(r), fg = front_float_from_half(g);
-            if (P.flags & kFrontFlipX) r = front_half_from_float(1.0f - fr);
-            if (P.flags & kFrontFlipY) g = front_half_from_float(1.0f - fg);
-        }
+        front_flip_hdr(r, g, P.flags);
         if (P.flags & kFrontNormalize) front_normalize_hdr(r, g, b);
         out[0] = r | (g << 16);
         out[1] = b | (a << 16);
@@ -161,8 +172,7 @@ ITW_HD void front_compose(u32 (&out)[2], const FrontParams& P, const u32 (&raw)[
     u32 g = (P.planes > 1) ? front_ldr_value(raw[1], P.depth, gamma) : missing;
     u32 b = (P.planes > 2) ? front_ldr_value(raw[2], P.depth, gamma) : missing;
     const u32 a = alpha ? front_ldr_value(raw[3], P.depth, gamma) : 255u;
-    if (P.flags & kFrontFlipX) r = 255u - r;                                                       // IP:1519-1527
-    if (P.flags & kFrontFlipY) g = 255u - g;
+    front_flip_ldr(r, g, P.flags);
     if (P.flags & kFrontNormalize) front_normalize_ldr(r, g, b);
     out[0] = r | (g << 8) | (b << 16) | (a << 24);
     out[1] = 0u;
@@ -176,6 +186,57 @@ ITW_HD void front_texel(u32 (&out)[2], const FrontParams& P, int x, int y)
     u32 raw[4] = {0u, 0u, 0u, 0u};
     for (int c = 0; c < P.planes; c++) raw[c] = front_load_raw(px + c * esize, P.depth);
     front_compose(out, P, raw);
+}
+
+// ---- mip levels from document layers (IP:1694-1850: CopyLayersIntoMipMaps, CopyFromLayerChannelIntoImage, FillLayerDataToWhite) ----
+// One level as the kernel writes it: the lw x lh top-left rectangle of one layer, staged as planar, tightly packed planes.
+constexpr int kLayerMaxLevels = 16;
+struct LayerLevel {
+    const uint8_t* plane[4];  // colour planes 0..channels-1; plane[3] = alpha, null = FillLayerDataToWhite
+    uint8_t* dst;             // the level's RGBA8 / RGBA16F surface
+    long long dst_stride;
+    long long first;          // first thread of this level in the launch
+    int lw, lh;               // texels read from the layer
+    int pw, ph;               // texels written (>= lw x lh: the edge is replicated, DoPaddingToMultiplesOf4)
+    int channels;             // 1..3
+};
+struct LayerLaunch {
+    LayerLevel lv[kLayerMaxLevels];
+    int count;
+    int depth;                // the document's: 8, 16 or 32
+    int hdr;                  // 1 = RGBA16F (BC6H), 0 = RGBA8
+    u32 flip;                 // kFrontFlipX / kFrontFlipY: level 0 only, applied after the copy (IP:2100-2105)
+};
+// FillLayerDataToWhite (IP:1664-1689) as the raw element the converters then read.  At depth 16 it stores
+// ConvertTo16Bit((unsigned8)255), the half 1.0 = 15360, which the 16-bit converters read as 15360 / 32768.
+ITW_HD u32 layer_white_raw(int depth)
+{
+    return depth == 8 ? 255u : (depth == 16 ? 15360u : 0x3F800000u);
+}
+// Texel (x, y) of one level: `px` holds the texel before the copy (RGBA8 in px[0]; RGBA16F as front_compose packs it) and
+// receives it after.  Planes c < channels and alpha are overwritten from the layer at the clamped position; the other planes
+// keep what they held.  RGBA8 targets at depth 32 always take the gamma step: the call binds ConvertTo8Bit(double, true).
+ITW_HD void layer_texel(u32 (&px)[2], const LayerLevel& L, int depth, bool hdr, u32 flip, int x, int y)
+{
+    const int sx = (x < L.lw) ? x : L.lw - 1, sy = (y < L.lh) ? y : L.lh - 1;
+    const int esize = depth >> 3;
+    const long long at = ((long long)sy * L.lw + sx) * esize;
+    u32 v[4];
+    if (hdr) { v[0] = px[0] & 0xFFFFu; v[1] = px[0] >> 16; v[2] = px[1] & 0xFFFFu; v[3] = px[1] >> 16; }
+    else { v[0] = px[0] & 255u; v[1] = (px[0] >> 8) & 255u; v[2] = (px[0] >> 16) & 255u; v[3] = px[0] >> 24; }
+    for (int c = 0; c < 4; c++) {
+        if (c < 3 && c >= L.channels) continue;
+        const u32 raw = (c < 3 || L.plane[3]) ? front_load_raw(L.plane[c] + at, depth) : layer_white_raw(depth);
+        v[c] = hdr ? front_hdr_value(raw, depth) : front_ldr_value(raw, depth, true);
+    }
+    if (hdr) {
+        front_flip_hdr(v[0], v[1], flip);
+        px[0] = v[0] | (v[1] << 16);
+        px[1] = v[2] | (v[3] << 16);
+    } else {
+        front_flip_ldr(v[0], v[1], flip);
+        px[0] = v[0] | (v[1] << 8) | (v[2] << 16) | (v[3] << 24);
+    }
 }
 
 #if defined(__CUDACC__)
@@ -211,6 +272,31 @@ __global__ void __launch_bounds__(256) normalize_kernel(uint8_t* __restrict__ pt
         u32 r = v & 255u, g = (v >> 8) & 255u, b = (v >> 16) & 255u;
         front_normalize_ldr(r, g, b);
         *p = r | (g << 8) | (b << 16) | (v & 0xFF000000u);
+    }
+}
+// Layers into mip levels: every level of `P` in ONE launch, one thread per written texel, the levels back to back in the
+// thread index (the small levels would otherwise be all launch overhead).  In place: a thread reads its own texel only when
+// planes survive the copy, and the generated levels' padding already replicates their edge, so no thread reads another's.
+__global__ void __launch_bounds__(256) layer_kernel(const __grid_constant__ LayerLaunch P)
+{
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    int k = 0;
+    while (k + 1 < P.count && i >= P.lv[k + 1].first) k++;
+    const LayerLevel& L = P.lv[k];
+    const long long j = i - L.first;
+    if (j >= (long long)L.pw * L.ph) return;
+    const int y = (int)(j / L.pw), x = (int)(j - (long long)y * L.pw);
+    uint8_t* p = L.dst + (long long)y * L.dst_stride + (long long)x * (P.hdr ? 8 : 4);
+    const bool keep = L.channels < 3;                       // alpha is always written
+    u32 px[2] = {0u, 0u};
+    if (P.hdr) {
+        if (keep) { const uint2 t = *reinterpret_cast<const uint2*>(p); px[0] = t.x; px[1] = t.y; }
+        layer_texel(px, L, P.depth, true, P.flip, x, y);
+        *reinterpret_cast<uint2*>(p) = make_uint2(px[0], px[1]);
+    } else {
+        if (keep) px[0] = *reinterpret_cast<const u32*>(p);
+        layer_texel(px, L, P.depth, false, P.flip, x, y);
+        *reinterpret_cast<u32*>(p) = px[0];
     }
 }
 // Fast path: one thread per TWO quads of four destination texels -> 128-bit stores; the 4 * planes * depth/8 source
