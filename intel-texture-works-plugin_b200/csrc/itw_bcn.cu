@@ -38,6 +38,53 @@ namespace {
 std::atomic<uint64_t> g_launches{0};
 std::atomic<int> g_default_device{-1};      // itw_set_devices() with ONE device: the process-wide default
 
+constexpr uint32_t fourcc(char a, char b, char c, char d)
+{
+    return (uint32_t)(uint8_t)a | ((uint32_t)(uint8_t)b << 8) | ((uint32_t)(uint8_t)c << 16) | ((uint32_t)(uint8_t)d << 24);
+}
+
+// What the library knows of each block-compressed DXGI format; every host file reads these facts from here.
+struct DxgiFormat {
+    int dxgi;
+    int bpb;                 // bytes per 4x4 block
+    int encoder;             // ITW_FORMAT_* that encodes it: _SRGB as its UNORM twin, BC6H_SF16 as BC6H (IntelPlugin.cpp:840-843)
+    int decoder;             // ITW_FORMAT_* of display_kernel / open_layer_kernel: _SRGB as its UNORM twin
+    bool srgb;
+    int twin;                // the _SRGB / UNORM twin; the format itself when it has none
+    bool hdr;
+    bool alpha_scan;         // the open path checks its alpha (HasAlpha; the plug-in excludes BC1)
+    uint32_t fourcc;         // legacy FourCC (DirectXTexDDS.cpp:479-486), 0 = the DX10 extension only
+    int family;              // front end: 0 RGBA8 colour, 1 BC4 / BC5, 2 BC6H
+    int texel_bytes;         // the encoder's input texel: RGBA8 or RGBA16F
+    bool itw;                // an ITW_FORMAT_* id, accepted by the format-taking entry points
+};
+constexpr DxgiFormat kDxgiFormats[] = {
+    // dxgi bpb enc dec  srgb   twin  hdr    scan   legacy FourCC           family texel itw
+    {71, 8,  71, 71, false, 72, false, false, fourcc('D', 'X', 'T', '1'), 0, 4, true},
+    {72, 8,  71, 71, true,  71, false, false, 0,                          0, 4, false},
+    {77, 16, 77, 77, false, 78, false, true,  fourcc('D', 'X', 'T', '5'), 0, 4, true},
+    {78, 16, 77, 77, true,  77, false, true,  0,                          0, 4, false},
+    {80, 8,  80, 80, false, 80, false, false, fourcc('B', 'C', '4', 'U'), 1, 4, true},
+    {83, 16, 83, 83, false, 83, false, false, fourcc('B', 'C', '5', 'U'), 1, 4, true},
+    {95, 16, 95, 95, false, 95, true,  false, 0,                          2, 8, true},
+    {96, 16, 95, 96, false, 96, true,  false, 0,                          2, 8, true},
+    {98, 16, 98, 98, false, 99, false, true,  0,                          0, 4, true},
+    {99, 16, 98, 98, true,  98, false, true,  0,                          0, 4, false},
+};
+// The row of a DXGI format, null when the library does not know it.
+inline const DxgiFormat* dxgi_format(int dxgi)
+{
+    for (const DxgiFormat& f : kDxgiFormats)
+        if (f.dxgi == dxgi) return &f;
+    return nullptr;
+}
+// The row of an ITW_FORMAT_* id, null for any other number.
+inline const DxgiFormat* itw_format(int format)
+{
+    const DxgiFormat* f = dxgi_format(format);
+    return f && f->itw ? f : nullptr;
+}
+
 inline int pad4(int v) { return (v + 3) & ~3; }
 template <typename T> inline T lvl(T v, int l) { v >>= l; return v ? v : 1; }      // size of mip level l
 inline bool pow2_dims(int w, int h) { return (w & (w - 1)) == 0 && (h & (h - 1)) == 0; }   // GenerateMipMaps then box-filters
@@ -171,19 +218,9 @@ bool is_device_pointer(const void* p)
     return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
 }
 
-struct FormatInfo { int bpb; int texel_bytes; };
-bool format_info(int format, FormatInfo& f)
-{
-    switch (format) {
-        case ITW_FORMAT_BC1: case ITW_FORMAT_BC4: f = {8, 4}; return true;
-        case ITW_FORMAT_BC3: case ITW_FORMAT_BC5: case ITW_FORMAT_BC7: f = {16, 4}; return true;
-        case ITW_FORMAT_BC6H: case ITW_FORMAT_BC6H_SF16: f = {16, 8}; return true;
-        default: return false;
-    }
-}
 // 0 = encode it, 1 = nothing to do, -1 = error.  Zero-height bands are legitimate: CompressImageMT hands them to the
 // threads beyond height/4 (win32Threads.cpp:217-230) and the reference's loops simply do not execute (kernel.ispc:600).
-int check_surface(const rgba_surface* s, const FormatInfo& f)
+int check_surface(const rgba_surface* s, const DxgiFormat& f)
 {
     if (!s) return fail("null surface");
     if (s->height == 0 && s->width >= 0 && (s->width & 3) == 0) return 1;
@@ -196,15 +233,17 @@ int check_surface(const rgba_surface* s, const FormatInfo& f)
 
 // An encoder resolved from (format, settings) before anything is enqueued: launch() can then fail only on a CUDA error.
 struct Encoder {
-    int format;                  // BC6H_SF16 is encoded by the unsigned encoder (IntelPlugin.cpp:840-843)
-    FormatInfo f;
+    int format;                  // the row's encoder: BC6H_SF16 is encoded by the unsigned encoder
+    DxgiFormat f;                // the row of `format`
     Bc7Params bc7;
     Bc6Params bc6;
 };
 int resolve_encoder(int format, const void* settings, Encoder& e)
 {
-    e.format = format == ITW_FORMAT_BC6H_SF16 ? ITW_FORMAT_BC6H : format;
-    if (!format_info(e.format, e.f)) return fail("unknown format");
+    const DxgiFormat* f = itw_format(format);
+    if (!f) return fail("unknown format");
+    e.format = f->encoder;
+    e.f = *itw_format(e.format);
     if (e.format == ITW_FORMAT_BC7) {
         if (!settings) return fail("CompressBlocksBC7: null settings");
         e.bc7 = bc7_params_from(*static_cast<const bc7_enc_settings*>(settings));
@@ -273,6 +312,58 @@ cudaError_t copy_rows_h2d(uint8_t* d, const void* h, size_t h_stride, size_t row
 {
     if (h_stride == row_bytes) return cudaMemcpyAsync(d, h, row_bytes * rows, cudaMemcpyHostToDevice, s);
     return cudaMemcpy2DAsync(d, row_bytes, h, h_stride, row_bytes, rows, cudaMemcpyHostToDevice, s);
+}
+// Stage a host pixel source in `buf` (tight rows); P.data / P.row_bytes are redirected.
+int stage_pixels(uint8_t*& buf, size_t& cap, FrontParams& P, cudaStream_t s)
+{
+    const size_t tight = (size_t)P.width * P.planes * (P.depth / 8);
+    if (grow(buf, cap, tight * P.height)) return -1;
+    ITW_CUDA(copy_rows_h2d(buf, P.data, (size_t)P.row_bytes, tight, (size_t)P.height, s));
+    P.data = buf;
+    P.row_bytes = (long long)tight;
+    return 0;
+}
+
+// The input of a staged launch: `bytes` at `ptr`, read in place when it is device memory aligned to `align` (0: never), else copied
+// to d_in first.  With `pixels` (ptr == pixels->data, align 1) it is a pixel source that stage_pixels copies to d_in from the host.
+struct StagedIn {
+    const uint8_t* ptr;
+    bool dev;
+    unsigned align;
+    size_t bytes;
+    FrontParams* pixels = nullptr;
+};
+// The output: `rows` rows of `row_bytes` at `ptr` / `pitch`, written in place when it is device memory with ptr and pitch aligned
+// to `align`, else written to d_out at `stage_pitch` and copied back in one 2-D copy.
+struct StagedOut {
+    uint8_t* ptr;
+    size_t pitch;
+    bool dev;
+    unsigned align;
+    size_t row_bytes, stage_pitch, rows;
+};
+// One kernel of a single-launch call: copy in, launch(d_src, d_dst, dst_stride, stream) bracketed by ev0 / ev1 for
+// itw_last_kernel_ms, copy out, drain.  Device operands order the call on the legacy default stream (the rule of CompressBlocks*).
+template <typename Launch>
+int run_staged(const StagedIn& in, const StagedOut& out, Launch&& launch)
+{
+    ThreadCtx& c = tls;
+    cudaStream_t s = (in.dev || out.dev) ? cudaStreamLegacy : c.stream;
+    const bool in_direct = in.dev && in.align && (reinterpret_cast<uintptr_t>(in.ptr) & (in.align - 1)) == 0;
+    const bool out_direct = out.dev && ((reinterpret_cast<uintptr_t>(out.ptr) | (uintptr_t)out.pitch) & (out.align - 1)) == 0;
+    if (!in_direct && !in.pixels && grow(c.d_in, c.d_in_cap, in.bytes)) return -1;
+    if (!out_direct && grow(c.d_out, c.d_out_cap, out.stage_pitch * out.rows)) return -1;
+    uint8_t* d_dst = out_direct ? out.ptr : c.d_out;
+    FirstError fe;
+    if (!in_direct && in.pixels) fe.step(stage_pixels(c.d_in, c.d_in_cap, *in.pixels, s));
+    else if (!in_direct) fe.step(cudaMemcpyAsync(c.d_in, in.ptr, in.bytes, in.dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s), "H2D");
+    if (fe.rc == 0) fe.step(cudaEventRecord(c.ev0, s), "cudaEventRecord");
+    if (fe.rc == 0) fe.step(launch(in_direct ? in.ptr : c.d_in, d_dst, (long long)(out_direct ? out.pitch : out.stage_pitch), s));
+    if (fe.rc == 0 && fe.step(cudaEventRecord(c.ev1, s), "cudaEventRecord")) c.timed = true;
+    if (fe.rc == 0 && !out_direct)
+        fe.step(cudaMemcpy2DAsync(out.ptr, out.pitch, d_dst, out.stage_pitch, out.row_bytes, out.rows,
+                                  out.dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s), "D2H");
+    return fe.drain({s});
 }
 
 // One surface encode on `s` through a staging pair: a host source is copied into d_in, then the launch, then the blocks go
@@ -561,9 +652,9 @@ int encode_any(int format, const rgba_surface* src, uint8_t* dst, const void* se
 {
     tls.err.clear();
     tls.pool_ms = -1.0f;
-    FormatInfo f;
-    if (!format_info(format, f)) return fail("unknown format");
-    const int chk = check_surface(src, f);
+    const DxgiFormat* f = itw_format(format);
+    if (!f) return fail("unknown format");
+    const int chk = check_surface(src, *f);
     if (chk) return chk < 0 ? -1 : 0;
     if (!dst) return fail("null dst");
     Encoder e;
@@ -609,40 +700,26 @@ int launch_decode(int format, const uint8_t* d_blocks, uint8_t* d_dst, int w, in
 int decode_any(int format, const uint8_t* blocks, const rgba_surface* dst)
 {
     tls.err.clear();
-    FormatInfo f;
-    if (!format_info(format, f)) return fail("unknown format");
-    if (const int chk = check_surface(dst, f)) return chk < 0 ? -1 : 0;
+    const DxgiFormat* f = itw_format(format);
+    if (!f) return fail("unknown format");
+    if (const int chk = check_surface(dst, *f)) return chk < 0 ? -1 : 0;
     if (!blocks) return fail("null blocks");
     if (ensure_ctx()) return -1;
-    ThreadCtx& c = tls;
-    const size_t row_bytes = (size_t)dst->width * f.texel_bytes;
-    const size_t in_bytes = (size_t)(dst->width >> 2) * (dst->height >> 2) * f.bpb;
-    const bool src_dev = is_device_pointer(blocks), dst_dev = is_device_pointer(dst->ptr);
-    cudaStream_t s = (src_dev || dst_dev) ? cudaStreamLegacy : c.stream;       // same ordering rule as encode_any
-    const bool src_direct = src_dev && (reinterpret_cast<uintptr_t>(blocks) & 15u) == 0;
-    const bool dst_direct = dst_dev && (((uintptr_t)dst->ptr | (uintptr_t)dst->stride) & 3u) == 0;
-    if (!src_direct && grow(c.d_in, c.d_in_cap, in_bytes)) return -1;
-    if (!dst_direct && grow(c.d_out, c.d_out_cap, row_bytes * dst->height)) return -1;
-    const uint8_t* d_blocks = src_direct ? blocks : c.d_in;
-    uint8_t* d_dst = dst_direct ? dst->ptr : c.d_out;
-    const long long stride = dst_direct ? dst->stride : (long long)row_bytes;
-    FirstError fe;
-    if (!src_direct) fe.step(cudaMemcpyAsync(c.d_in, blocks, in_bytes, src_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s), "H2D");
-    if (fe.rc == 0) fe.step(cudaEventRecord(c.ev0, s), "cudaEventRecord");
-    if (fe.rc == 0) fe.step(launch_decode(format, d_blocks, d_dst, dst->width, dst->height, stride, s));
-    if (fe.rc == 0 && fe.step(cudaEventRecord(c.ev1, s), "cudaEventRecord")) c.timed = true;
-    if (fe.rc == 0 && !dst_direct)
-        fe.step(cudaMemcpy2DAsync(dst->ptr, (size_t)dst->stride, d_dst, row_bytes, row_bytes, (size_t)dst->height,
-                                  dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s), "D2H");
-    return fe.drain({s});
+    const size_t row_bytes = (size_t)dst->width * f->texel_bytes;
+    const size_t in_bytes = (size_t)(dst->width >> 2) * (dst->height >> 2) * f->bpb;
+    const StagedIn in{blocks, is_device_pointer(blocks), 16, in_bytes};
+    const StagedOut out{dst->ptr, (size_t)dst->stride, is_device_pointer(dst->ptr), 4, row_bytes, row_bytes, (size_t)dst->height};
+    return run_staged(in, out, [&](const uint8_t* d_blocks, uint8_t* d_dst, long long stride, cudaStream_t s) {
+        return launch_decode(f->decoder, d_blocks, d_dst, dst->width, dst->height, stride, s);
+    });
 }
 
 
 // ---- pixel-format front end (frontend.cuh) ----
 int front_params(FrontParams& P, int format, const itw_pixel_source* src, uint32_t flags)
 {
-    FormatInfo f;
-    if (!format_info(format, f)) return fail("unknown format");
+    const DxgiFormat* f = itw_format(format);
+    if (!f) return fail("unknown format");
     if (!src || !src->data) return fail("null pixel source");
     if (src->width <= 0 || src->height <= 0) return fail("pixel source: width/height must be positive");
     if (pad4(src->height) > 65535) return fail("pixel source: height above 65532");      // one grid row per (padded) output row
@@ -654,7 +731,7 @@ int front_params(FrontParams& P, int format, const itw_pixel_source* src, uint32
     const long long row_bytes = src->row_bytes ? src->row_bytes : tight;
     if (row_bytes < tight) return fail("pixel source: row_bytes smaller than a texel row");
     if ((reinterpret_cast<uintptr_t>(src->data) | (uintptr_t)row_bytes) & (uintptr_t)(esize - 1)) return fail("pixel source: misaligned elements");
-    const int family = (format == ITW_FORMAT_BC6H || format == ITW_FORMAT_BC6H_SF16) ? 2 : ((format == ITW_FORMAT_BC4 || format == ITW_FORMAT_BC5) ? 1 : 0);
+    const int family = f->family;
     if (flags & ITW_FRONT_HAS_ALPHA) {
         // the converters read plane 3 (IntelPlugin.cpp:310, :758 ...); the 32-bit HDR one reads plane 2 (:361)
         const int need = (family == 2 && src->depth == 32) ? 3 : 4;
@@ -690,43 +767,23 @@ int launch_front(const FrontParams& P, uint8_t* d_dst, int dw, int dh, long long
     ITW_CUDA(cudaGetLastError());
     return 0;
 }
-// Stage a host pixel source in `buf` (tight rows); P.data / P.row_bytes are redirected.
-int stage_pixels(uint8_t*& buf, size_t& cap, FrontParams& P, cudaStream_t s)
-{
-    const size_t tight = (size_t)P.width * P.planes * (P.depth / 8);
-    if (grow(buf, cap, tight * P.height)) return -1;
-    ITW_CUDA(copy_rows_h2d(buf, P.data, (size_t)P.row_bytes, tight, (size_t)P.height, s));
-    P.data = buf;
-    P.row_bytes = (long long)tight;
-    return 0;
-}
 int convert_any(int format, const itw_pixel_source* src, uint32_t flags, const rgba_surface* dst)
 {
     tls.err.clear();
     FrontParams P;
     if (front_params(P, format, src, flags)) return -1;
     if (!dst || !dst->ptr) return fail("null surface");
-    const int texel = (P.family == 2) ? 8 : 4;
+    const int texel = itw_format(format)->texel_bytes;
     if (!((dst->width == P.width && dst->height == P.height) || (dst->width == pad4(P.width) && dst->height == pad4(P.height))))
         return fail("itw_convert_pixels: dst must have the source size or that size rounded up to multiples of 4");
     if ((long long)dst->stride < (long long)dst->width * texel) return fail("surface stride smaller than a texel row");
     if (ensure_ctx()) return -1;
-    ThreadCtx& c = tls;
-    const bool src_dev = is_device_pointer(P.data), dst_dev = is_device_pointer(dst->ptr);
-    cudaStream_t s = (src_dev || dst_dev) ? cudaStreamLegacy : c.stream;
-    const bool dst_direct = dst_dev && (((uintptr_t)dst->ptr | (uintptr_t)dst->stride) & (uintptr_t)(texel - 1)) == 0;
     const size_t row_bytes = (size_t)dst->width * texel;
-    if (!dst_direct && grow(c.d_out, c.d_out_cap, row_bytes * dst->height)) return -1;
-    uint8_t* d_dst = dst_direct ? dst->ptr : c.d_out;
-    FirstError fe;
-    if (!src_dev) fe.step(stage_pixels(c.d_in, c.d_in_cap, P, s));
-    if (fe.rc == 0) fe.step(cudaEventRecord(c.ev0, s), "cudaEventRecord");
-    if (fe.rc == 0) fe.step(launch_front(P, d_dst, dst->width, dst->height, dst_direct ? dst->stride : (long long)row_bytes, s));
-    if (fe.rc == 0 && fe.step(cudaEventRecord(c.ev1, s), "cudaEventRecord")) c.timed = true;
-    if (fe.rc == 0 && !dst_direct)
-        fe.step(cudaMemcpy2DAsync(dst->ptr, (size_t)dst->stride, d_dst, row_bytes, row_bytes, (size_t)dst->height,
-                                  dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s), "D2H");
-    return fe.drain({s});
+    const StagedIn in{P.data, is_device_pointer(P.data), 1, 0, &P};
+    const StagedOut out{dst->ptr, (size_t)dst->stride, is_device_pointer(dst->ptr), (unsigned)texel, row_bytes, row_bytes, (size_t)dst->height};
+    return run_staged(in, out, [&](const uint8_t*, uint8_t* d_dst, long long stride, cudaStream_t s) {
+        return launch_front(P, d_dst, dst->width, dst->height, stride, s);
+    });
 }
 // convert + pad + encode; the intermediate surface never leaves the GPU
 int encode_pixels_any(int format, const itw_pixel_source* src, uint32_t flags, const void* settings, uint8_t* dst)
@@ -786,16 +843,16 @@ void CompressBlocksBC5(const rgba_surface* src, uint8_t* dst) { encode_any(ITW_F
 
 int itw_bytes_per_block(int format)
 {
-    FormatInfo f;
-    return format_info(format, f) ? f.bpb : 0;
+    const DxgiFormat* f = itw_format(format);
+    return f ? f->bpb : 0;
 }
 
 int itw_encode_device(int format, const rgba_surface* src, uint8_t* dst, const void* settings, void* cuda_stream)
 {
     tls.err.clear();
-    FormatInfo f;
-    if (!format_info(format, f)) return fail("unknown format");
-    if (const int chk = check_surface(src, f)) return chk < 0 ? -1 : 0;
+    const DxgiFormat* f = itw_format(format);
+    if (!f) return fail("unknown format");
+    if (const int chk = check_surface(src, *f)) return chk < 0 ? -1 : 0;
     if (!dst) return fail("null dst");
     if (reinterpret_cast<uintptr_t>(dst) & 15u) return fail("itw_encode_device: dst must be 16-byte aligned");
     Encoder e;
