@@ -476,6 +476,54 @@ int itw_dds_open_layout(itw_dds_open_info* info, uint32_t options);
  * too small, info not laid out): on failure dst is untouched.  Returns 0 on success. */
 int itw_dds_read_layer(const uint8_t* file, size_t size, const itw_dds_open_info* info, int call, void* dst, int64_t row_bytes);
 
+/* ---------------------------------------------------------------------------------------------
+ * Section 10 -- cube maps from the document: the save dialog's two cube texture types, CUBEMAP_CROSSED and CUBEMAP_LAYERS
+ * (IntelPlugin.cpp:44-65), through DoWriteDDS (:2062-2171) and GetCompressedImageForPreview (:933-1080), with the dialog's
+ * "set mip level" option (IsCubeMapWithSetMipLevelOverride, :1172-1179).
+ *   cross   ConvertToCubeMapFromCross (:1200-1265): six W x H cells of one document.  A horizontal 4x3 cross (doc width >= doc
+ *           height) gives W = doc_width / 4, H = doc_height / 3; a vertical 3x4 cross gives W = doc_width / 3, H = doc_height / 4 and
+ *           takes -Z from cell (1, 3), unrotated.  For a 1/3/7 _SRGB encoding with mip maps the document scratch is
+ *           R8G8B8A8_UNORM_SRGB (:152-154) and the cube scratch R8G8B8A8_UNORM (:1240-1246), so CopyRectangle LINEARISES r, g, b of
+ *           every cell (XMColorSRGBToRGB, then the UNORM8 store); otherwise the cells are copied as converted.
+ *   layers  ConvertToCubeMapFromLayers (:1270-1416): face i starts all zero (InitializeCube) and is filled from the layer named
+ *           +X, -X, +Y, -Y, +Z, -Z by the per-texel rules of itw_dds_encode_layers (channels c < channel_count, alpha from the
+ *           layer when ITW_FRONT_HAS_ALPHA is set and `alpha` is not NULL, else white -- 119 / 0x3780 at depth 16 -- and RGBA8
+ *           targets always gamma-correct 32-bit layers).  W x H = the document size.  A face with no layer stays zero.
+ * The chain is filtered as the cube scratch is: R8G8B8A8_UNORM for every 8-bit format (_SRGB included), RGBA16F for BC6H.
+ * ------------------------------------------------------------------------------------------- */
+enum { ITW_CUBE_CROSS = 0, ITW_CUBE_LAYERS = 1 };
+typedef struct itw_cube_options {
+    uint32_t dxgi_format;  /* the plug-in's cube columns: 71/72 BC1, 77/78 BC3, 95 BC6H_UF16, 98/99 BC7 (BC4, BC5 and BC6H_SF16 are
+                              refused: the plug-in offers no cube of them, or builds it as RGBA8)                                    */
+    int32_t  source;       /* ITW_CUBE_CROSS: the document is the cross; ITW_CUBE_LAYERS: six face layers                          */
+    int32_t  mip_maps;     /* 0 / 1: the dialog's MipMapTypeIndex != NONE (AUTOGEN or FROM_LAYERS: DoMipMaps, :2056)               */
+    int32_t  mip_level;    /* -1, or L: the set mip level.  The file is then the one-level cube of level L of every face
+                              (SaveCubeMipLevelToDDSFile, :1856-1871); 0 <= L < max(W, H).bit_length()                            */
+} itw_cube_options;
+/* Pure arithmetic, no CUDA call: the face size (*face_width / *face_height, may be NULL) and the desc of the file the save writes.
+ * Without L: W x H, the full chain with mip_maps, else 1 level.  With L: max(1, W >> L) x max(1, H >> L), 1 level.  Always array_size 6,
+ * is_cubemap 1.  Returns the file size; 0 with an error text when the options or the document size are refused (a cross smaller
+ * than one texel per face). */
+size_t itw_cube_layout(const itw_cube_options* o, int doc_width, int doc_height, itw_dds_desc* desc, int* face_width, int* face_height);
+/* DoWriteDDS for the two cube types.  `document` = the composite: its texels are read only for ITW_CUBE_CROSS (`data` may be NULL for
+ * ITW_CUBE_LAYERS, where it gives the size and the depth).  `faces` = six itw_layer_source in +X,-X,+Y,-Y,+Z,-Z order, channels[0] NULL
+ * for a face without a layer of that name; ignored for a cross (may be NULL).  Each face layer is read whole: W x H planes of the
+ * document's depth.  `flags`: ITW_FRONT_HAS_ALPHA and ITW_FRONT_GAMMA only (the plug-in flips and normalises normal maps only,
+ * :2103, :2151).  With L only levels 0..L are built and only level L is encoded (the plug-in encodes the whole chain and keeps
+ * level L; the bytes of level L are the same).  `settings` as for itw_encode_device.  Every operand may be host or device memory
+ * (the ordering rule of CompressBlocks*); synchronous.  Returns the file size, or 0 with an error text and `file` untouched when an
+ * argument is refused (nothing is enqueued then). */
+size_t itw_dds_encode_cube(const itw_cube_options* o, const itw_pixel_source* document, const itw_layer_source* faces, uint32_t flags,
+                           const void* settings, uint8_t* file, size_t capacity);
+/* GetCompressedImageForPreview for the two cube types, with itw_preview_pixels' display rules (target, shown format).  A cross without
+ * L is the 2-D preview of the whole document (:966 does not fire): itw_preview_pixels with count 1.  Otherwise the faces are built
+ * as for a save but never linearised (the preview's CopyDataForEncoding passes DoMipMaps = false, :957), the chain runs to L when
+ * set, and the horizontal cross of level L (4 wL x 3 hL, cells without a face zero, :1421-1501) is padded, encoded and decompressed
+ * into `display`, which must have the size of the document (cross without L) or of that cross.  *compressed_bytes (may be NULL)
+ * receives the size of the encoded image.  Rejections as for itw_dds_encode_cube; `display` is then untouched.  Returns 0 on success. */
+int itw_preview_cube(const itw_cube_options* o, const itw_pixel_source* document, const itw_layer_source* faces, uint32_t flags,
+                     const void* settings, const rgba_surface* display, size_t* compressed_bytes);
+
 #ifdef __cplusplus
 }
 #endif

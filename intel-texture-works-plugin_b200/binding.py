@@ -52,7 +52,7 @@ EXPORTS = (["CompressBlocksBC1", "CompressBlocksBC3", "CompressBlocksBC4", "Comp
             "CompressImageMT", "CompressImageST", "CompressImageBC1", "CompressImageBC3",
             "itw_shard_plan_make", "itw_shard_unique_id", "itw_shard_init", "itw_shard_finalize", "itw_encode_mip_chain_sharded",
             "itw_decompress", "itw_preview_pixels", "itw_dds_open", "itw_dds_open_layout", "itw_dds_read_layer",
-            "itw_dds_encode_layers"]
+            "itw_dds_encode_layers", "itw_cube_layout", "itw_dds_encode_cube", "itw_preview_cube"]
            + ["CompressImageBC7_" + p for p in BC7_PROFILES] + ["CompressImage" + p.replace("bc6h_", "BC6H_") for p in BC6H_PROFILES]
            + ["GetProfile_" + p for p in BC7_PROFILES + BC6H_PROFILES])
 
@@ -82,6 +82,13 @@ class DdsOpenInfo(ctypes.Structure):         # include/itw_bcn.h section 9
 
 
 OPEN_SEPARATE_ALPHA, OPEN_MIPS = 1, 2
+
+
+class CubeOptions(ctypes.Structure):          # include/itw_bcn.h section 10
+    _fields_ = [("dxgi_format", ctypes.c_uint32), ("source", ctypes.c_int32), ("mip_maps", ctypes.c_int32), ("mip_level", ctypes.c_int32)]
+
+
+CUBE_CROSS, CUBE_LAYERS = 0, 1
 
 
 class ShardPlan(ctypes.Structure):            # include/itw_bcn.h section 7
@@ -323,6 +330,88 @@ class ItwBcn(EncoderApi):
             self.check()
             raise RuntimeError("itw_dds_encode_file failed")
         return out
+
+    def cube_layout(self, options, doc_width, doc_height):
+        """itw_cube_layout: (file size, DdsDesc, face width, face height); size 0 (and the error text) when refused."""
+        f = self.lib.itw_cube_layout
+        f.restype = ctypes.c_size_t
+        f.argtypes = [ctypes.POINTER(CubeOptions), ctypes.c_int, ctypes.c_int, ctypes.POINTER(DdsDesc), ctypes.POINTER(ctypes.c_int),
+                      ctypes.POINTER(ctypes.c_int)]
+        d, fw, fh = DdsDesc(), ctypes.c_int(0), ctypes.c_int(0)
+        n = f(ctypes.byref(options), doc_width, doc_height, ctypes.byref(d), ctypes.byref(fw), ctypes.byref(fh))
+        return n, d, fw.value, fh.value
+
+    @staticmethod
+    def cube_faces(faces, dtype, keep):
+        """Six LayerSource from `faces`: per face None (no layer of that name) or (channels, alpha) as dds_encode_layers takes them."""
+        arr = (LayerSource * 6)()
+        for i, face in enumerate(faces):
+            if face is None:
+                continue
+            channels, alpha = face
+            planes = [np.ascontiguousarray(c, dtype) for c in channels]
+            a = None if alpha is None else np.ascontiguousarray(alpha, dtype)
+            keep += planes + [a]
+            arr[i].channel_count = len(planes)
+            for c, pl in enumerate(planes):
+                arr[i].channels[c] = pl.ctypes.data
+            arr[i].alpha = None if a is None else a.ctypes.data
+        return arr
+
+    def dds_encode_cube(self, options, document, faces=None, flags=0, settings=None):
+        """itw_dds_encode_cube: `document` = host numpy H x W x planes array (the cross, or the composite that gives the size and depth
+        of a layer cube); `faces` = six entries as cube_faces takes them (layer cubes only)."""
+        doc = np.ascontiguousarray(document)
+        n = self.cube_layout(options, doc.shape[1], doc.shape[0])[0]
+        if not n:
+            raise ValueError("itw_cube_layout refused the options: " + self.last_error())
+        keep = []
+        arr = self.cube_faces(faces, doc.dtype, keep) if faces is not None else None
+        src = PixelSource(doc.ctypes.data, doc.shape[1], doc.shape[0], doc.shape[2], doc.itemsize * 8, 0)
+        out = np.zeros(n, np.uint8)
+        sp = ctypes.cast(ctypes.byref(settings), ctypes.c_void_p) if settings is not None else None
+        got = self.dds_encode_cube_raw(options, src, arr, flags, sp, out.ctypes.data, n)
+        if got != n:
+            raise RuntimeError("itw_dds_encode_cube failed: " + self.last_error())
+        return out
+
+    def dds_encode_cube_raw(self, options, document, faces, flags, settings_ptr, file_ptr, capacity):
+        """itw_dds_encode_cube on ctypes structures and raw addresses; returns the file size (0 on error)."""
+        f = self.lib.itw_dds_encode_cube
+        f.restype = ctypes.c_size_t
+        f.argtypes = [ctypes.POINTER(CubeOptions), ctypes.POINTER(PixelSource), ctypes.POINTER(LayerSource), ctypes.c_uint32, ctypes.c_void_p,
+                      ctypes.c_void_p, ctypes.c_size_t]
+        return f(ctypes.byref(options), ctypes.byref(document), faces, flags, settings_ptr, file_ptr, capacity)
+
+    def preview_cube(self, options, document, faces=None, flags=0, settings=None):
+        """itw_preview_cube on host arrays (as dds_encode_cube) -> (display image, compressed bytes).  The display is the document
+        (a cross without a set level) or the 4 wL x 3 hL cross; float32 for BC6H at depth 32, uint8 otherwise."""
+        doc = np.ascontiguousarray(document)
+        n, d, fw, fh = self.cube_layout(options, doc.shape[1], doc.shape[0])
+        if not n:
+            raise ValueError("itw_cube_layout refused the options: " + self.last_error())
+        if options.source == CUBE_CROSS and options.mip_level < 0:
+            w, h = doc.shape[1], doc.shape[0]
+        else:
+            w, h = 4 * d.width, 3 * d.height
+        img = np.zeros((h, w, 4), np.float32 if (options.dxgi_format == 95 and doc.itemsize == 4) else np.uint8)
+        keep = []
+        arr = self.cube_faces(faces, doc.dtype, keep) if faces is not None else None
+        src = PixelSource(doc.ctypes.data, doc.shape[1], doc.shape[0], doc.shape[2], doc.itemsize * 8, 0)
+        sp = ctypes.cast(ctypes.byref(settings), ctypes.c_void_p) if settings is not None else None
+        size = ctypes.c_size_t(0)
+        rc = self.preview_cube_raw(options, src, arr, flags, sp, RgbaSurface(img.ctypes.data, w, h, img.strides[0]), ctypes.byref(size))
+        if rc != 0:
+            raise RuntimeError("itw_preview_cube failed: " + self.last_error())
+        return img, size.value
+
+    def preview_cube_raw(self, options, document, faces, flags, settings_ptr, display, size_ref):
+        """itw_preview_cube on ctypes structures; returns its status."""
+        f = self.lib.itw_preview_cube
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.POINTER(CubeOptions), ctypes.POINTER(PixelSource), ctypes.POINTER(LayerSource), ctypes.c_uint32, ctypes.c_void_p,
+                      ctypes.POINTER(RgbaSurface), ctypes.POINTER(ctypes.c_size_t)]
+        return f(ctypes.byref(options), ctypes.byref(document), faces, flags, settings_ptr, ctypes.byref(display), size_ref)
 
     def decompress(self, dxgi_format, blocks, width, height, target):
         """itw_decompress: host blocks -> H x W x 4 image of `target` (uint8 for 28 / 29, float32 for 2)."""

@@ -37,8 +37,7 @@
 namespace itw {
 
 ITW_TABLE_DECL(uint32_t, srgb_in_threshold, 255)
-ITW_TABLE_DECL(uint32_t, srgb_in_byte, 64)
-ITW_TABLE_DECL(uint32_t, srgb_out_byte, 64)
+ITW_TABLE_DECL(uint32_t, srgb_out_byte, 64)      // srgb_in_byte and byte_table: frontend.cuh
 
 enum DisplayRule { kDisplayPlain = 0, kDisplaySrgbIn = 1, kDisplaySrgbOut = 2, kDisplayHdrUnorm = 3, kDisplayHdrFloat = 4 };
 
@@ -53,7 +52,6 @@ ITW_HD u32 threshold_count(const uint32_t* T, float f)
         if ((int)T[k + s - 1] <= b) k += s;
     return (u32)k;
 }
-ITW_HD u32 byte_table(const uint32_t* T, u32 b) { return (T[b >> 2] >> (8 * (b & 3u))) & 255u; }
 
 struct SrgbInStore { ITW_HD static u32 of(float x) { return threshold_count(ITW_TABLE(srgb_in_threshold), x); } };
 struct SrgbOutStore { ITW_HD static u32 of(float x) { return threshold_count(ITW_TABLE(linear_threshold), x); } };

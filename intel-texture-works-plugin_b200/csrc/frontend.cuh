@@ -16,10 +16,14 @@
 #pragma once
 #include "itw_device.cuh"
 #include "gamma_table.cuh"
+#include "display_tables.cuh"
 
 namespace itw {
 
 ITW_TABLE_DECL(uint32_t, gamma_threshold, 255)
+// byte b -> the stored byte of XMColorSRGBToRGB(b * (1/255)) (tools/gen_display_tables.py); shared with display.cuh
+ITW_TABLE_DECL(uint32_t, srgb_in_byte, 64)
+ITW_HD u32 byte_table(const uint32_t* T, u32 b) { return (T[b >> 2] >> (8 * (b & 3u))) & 255u; }
 
 struct FrontParams {
     const uint8_t* data;
@@ -184,7 +188,9 @@ ITW_HD void front_texel(u32 (&out)[2], const FrontParams& P, int x, int y)
     const int esize = P.depth >> 3;
     const uint8_t* px = P.data + (long long)sy * P.row_bytes + (long long)sx * P.planes * esize;
     u32 raw[4] = {0u, 0u, 0u, 0u};
-    for (int c = 0; c < P.planes; c++) raw[c] = front_load_raw(px + c * esize, P.depth);
+#pragma unroll
+    for (int c = 0; c < 4; c++)                               // constant indices: raw stays in registers
+        if (c < P.planes) raw[c] = front_load_raw(px + c * esize, P.depth);
     front_compose(out, P, raw);
 }
 
@@ -236,6 +242,35 @@ ITW_HD void layer_texel(u32 (&px)[2], const LayerLevel& L, int depth, bool hdr, 
     } else {
         front_flip_ldr(v[0], v[1], flip);
         px[0] = v[0] | (v[1] << 8) | (v[2] << 16) | (v[3] << 24);
+    }
+}
+
+// ---- cube maps from a cross document (IP:1200-1265: ConvertToCubeMapFromCross) ----
+// Cells (column, row) of +X,-X,+Y,-Y,+Z,-Z: the horizontal 4x3 cross (IP:1211) and the vertical 3x4 one, where -Z moves to (1, 3)
+// and is copied unrotated (IP:1225-1226).  Host side: the launch carries the six texel origins.
+constexpr int kCubeCells[2][6][2] = {{{2, 1}, {0, 1}, {1, 0}, {1, 2}, {1, 1}, {3, 1}}, {{2, 1}, {0, 1}, {1, 0}, {1, 2}, {1, 1}, {1, 3}}};
+struct CubeCross {
+    FrontParams P;            // the whole document (flags: alpha, gamma)
+    uint8_t* dst;             // level 0 of face 0; face f at dst + f * face_bytes, w x h texels, rows `stride` apart
+    long long face_bytes, stride;
+    int w, h;                 // face size
+    int origin[6][2];         // texel origin of each face's cell in the document
+    int linear;               // RGBA8 only: the cells are linearised (XMColorSRGBToRGB on r, g, b; alpha passes)
+};
+// Texel (x, y) of face `face`: the front end at the cell's texel, then -- for an _SRGB encoding with mip maps, whose document scratch is
+// R8G8B8A8_UNORM_SRGB while the cube scratch is R8G8B8A8_UNORM (IP:152-154, :1240-1246) -- CopyRectangle's conversion (DirectXTexMisc.cpp:
+// 174-274: _LoadScanline, _ConvertScanline with TEX_FILTER_SRGB_IN, the UNORM8 store), which is a byte -> byte map per colour channel.
+ITW_HD void cube_texel(u32 (&out)[2], const CubeCross& C, int face, int x, int y)
+{
+    int ox = 0, oy = 0;
+#pragma unroll
+    for (int f = 0; f < 6; f++)                               // constant indices: the table stays in the parameter space, no stack copy
+        if (f == face) { ox = C.origin[f][0]; oy = C.origin[f][1]; }
+    front_texel(out, C.P, ox + x, oy + y);
+    if (C.linear) {
+        const u32 v = out[0];
+        out[0] = byte_table(ITW_TABLE(srgb_in_byte), v & 255u) | (byte_table(ITW_TABLE(srgb_in_byte), (v >> 8) & 255u) << 8) |
+                 (byte_table(ITW_TABLE(srgb_in_byte), (v >> 16) & 255u) << 16) | (v & 0xFF000000u);
     }
 }
 
@@ -298,6 +333,18 @@ __global__ void __launch_bounds__(256) layer_kernel(const __grid_constant__ Laye
         layer_texel(px, L, P.depth, false, P.flip, x, y);
         *reinterpret_cast<u32*>(p) = px[0];
     }
+}
+// Level 0 of all six faces of a cross document in ONE launch: blockIdx.z = face, blockIdx.y = row, one thread per texel.  Per texel
+// planes*depth/8 B in, 4 / 8 B out; the document is read once in total (the cells do not overlap).
+__global__ void __launch_bounds__(256) cube_faces_kernel(const __grid_constant__ CubeCross C)
+{
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y, face = blockIdx.z;
+    if (x >= C.w || y >= C.h) return;
+    u32 out[2];
+    cube_texel(out, C, face, x, y);
+    uint8_t* row = C.dst + face * C.face_bytes + (long long)y * C.stride;
+    if (C.P.family == 2) *reinterpret_cast<uint2*>(row + (long long)x * 8) = make_uint2(out[0], out[1]);
+    else *reinterpret_cast<u32*>(row + (long long)x * 4) = out[0];
 }
 // Fast path: one thread per TWO quads of four destination texels -> 128-bit stores; the 4 * planes * depth/8 source
 // bytes of a quad are contiguous and 4-byte aligned, and are fetched as 32-bit words into registers (all indices are

@@ -1098,3 +1098,4 @@ int itw_bc7_phase_clocks(void* out, size_t bytes)
 #include "itw_shard.inc"
 #include "itw_preview.inc"
 #include "itw_open.inc"
+#include "itw_cube.inc"
