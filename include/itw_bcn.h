@@ -524,6 +524,46 @@ size_t itw_dds_encode_cube(const itw_cube_options* o, const itw_pixel_source* do
 int itw_preview_cube(const itw_cube_options* o, const itw_pixel_source* document, const itw_layer_source* faces, uint32_t flags,
                      const void* settings, const rgba_surface* display, size_t* compressed_bytes);
 
+/* ---------------------------------------------------------------------------------------------
+ * Section 11 -- the preview dialog: the compressed pane of "mip maps from layers" (GetCompressedImageForPreview with
+ * IsMipMapsDefinedByLayer, IntelPlugin.cpp:986-993) and the dialog's view of a pane (FetchPreviewRGB, :487-739), which
+ * PreviewDialog::updatePreviewBuffer (PreviewDialog.cpp:260-274) calls for both panes on every repaint, pan, zoom or channel toggle.
+ * ------------------------------------------------------------------------------------------- */
+/* itw_preview_pixels of a 2-D document whose level 0 comes from layer 0, in the plug-in's order: CopyDataForEncoding (no mip maps,
+ * so the scratch is R8G8B8A8_UNORM even for _SRGB encodings) -> CopyLayersIntoMipMaps(..., 0, 1): layer 0 overwrites the converted
+ * composite with the per-texel rules of itw_dds_encode_layers (white alpha when the layer has none -- 15360 at depth 16 -- and the
+ * v^(1/2.2) step for 32-bit layers into RGBA8) -> FlipXYChannelNormalMap (so _SRGB encodings are flipped too, unlike the save path)
+ * -> NormalizeNormalMapChain -> pad -> encode -> display decompress, with itw_preview_pixels' display rules (target, shown format).
+ * `layer0` is read whole: composite->width x composite->height planes of the composite's depth.  *compressed_bytes (may be NULL)
+ * receives the slice pitch of level 0.  Every operand may be host or device memory; synchronous.  Rejections (those of
+ * itw_dds_encode_layers for layer 0 and of itw_preview_pixels) happen before anything is enqueued and leave `display` untouched.
+ * Returns 0 on success. */
+int itw_preview_layers(int dxgi_format, const itw_pixel_source* composite, const itw_layer_source* layer0, uint32_t flags,
+                       const void* settings, const rgba_surface* display, size_t* compressed_bytes);
+
+enum { ITW_VIEW_RED = 0x4, ITW_VIEW_GREEN = 0x8, ITW_VIEW_BLUE = 0x10, ITW_VIEW_ALPHA = 0x20 };   /* PREVIEW_CHANNEL_* values */
+typedef struct itw_view {
+    int32_t  width, height;   /* the dialog buffer: width*height packed RGB8 texels                                    */
+    int32_t  x, y;            /* previewOffsetX / Y                                                                      */
+    double   zoom;            /* what the dialog passes: 1.f / previewZoom                                               */
+    int32_t  mip_level;       /* SetMipLevel ? MipLevel : 0; zoom is divided by 1 << mip_level as at :503-504            */
+    uint32_t channels;        /* ITW_VIEW_* mask; 0 = RGB (:492-493)                                                    */
+    uint32_t matte;           /* 0x00BBGGRR                                                                              */
+} itw_view;
+/* FetchPreviewRGB's sampling into `dst` (view->width * view->height * 3 bytes, rows tightly packed).  `source` is the document
+ * (depth 8, 16 or 32, planes 1..4, any row_bytes) or a pane: the display of itw_preview_pixels / _layers / _cube as R8G8B8A8_UNORM
+ * (depth 8, planes 4) or R32G32B32A32_FLOAT (depth 32, planes 4); the plug-in switches on depth and format together, so those share
+ * the branches of depths 8 and 32.  Dialog texel (xt, yt) shows source texel (int((xt + x) * z), int((yt + y) * z)), z = zoom /
+ * (1 << mip_level), in double and truncated toward zero (an offset in (-1, 0) lands on texel 0); texels outside the source get the
+ * matte bytes.  Channels (:585-624): pure R, G, B or A show grey, in a mixture alpha takes the blue slot, a channel beyond `planes`
+ * shows 0.  Stores: depth 8 the byte, depth 16 FloatToByte(v / 32768.0), depth 32 FloatToByte((double)f) without gamma.
+ * Not covered: the R16G16B16A16_FLOAT branch (no pane is built in that format) and `exposure` other than 1 (InitData sets 1,
+ * :1889, and nothing changes it).  Either side may be host or device memory (a host source is copied whole; device operands: the
+ * ordering rule of CompressBlocks*); synchronous.  Every argument is checked before anything is enqueued (null pointers, a depth,
+ * planes or row_bytes the source cannot have, a non-positive view size, a zoom that is not positive and finite, mip_level outside
+ * 0..30, channel bits other than ITW_VIEW_*): `dst` is then untouched.  Returns 0 on success. */
+int itw_preview_view(const itw_pixel_source* source, const itw_view* view, uint8_t* dst);
+
 #ifdef __cplusplus
 }
 #endif

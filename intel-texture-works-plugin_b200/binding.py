@@ -52,7 +52,7 @@ EXPORTS = (["CompressBlocksBC1", "CompressBlocksBC3", "CompressBlocksBC4", "Comp
             "CompressImageMT", "CompressImageST", "CompressImageBC1", "CompressImageBC3",
             "itw_shard_plan_make", "itw_shard_unique_id", "itw_shard_init", "itw_shard_finalize", "itw_encode_mip_chain_sharded",
             "itw_decompress", "itw_preview_pixels", "itw_dds_open", "itw_dds_open_layout", "itw_dds_read_layer",
-            "itw_dds_encode_layers", "itw_cube_layout", "itw_dds_encode_cube", "itw_preview_cube"]
+            "itw_dds_encode_layers", "itw_cube_layout", "itw_dds_encode_cube", "itw_preview_cube", "itw_preview_layers", "itw_preview_view"]
            + ["CompressImageBC7_" + p for p in BC7_PROFILES] + ["CompressImage" + p.replace("bc6h_", "BC6H_") for p in BC6H_PROFILES]
            + ["GetProfile_" + p for p in BC7_PROFILES + BC6H_PROFILES])
 
@@ -89,6 +89,14 @@ class CubeOptions(ctypes.Structure):          # include/itw_bcn.h section 10
 
 
 CUBE_CROSS, CUBE_LAYERS = 0, 1
+
+
+class View(ctypes.Structure):                 # include/itw_bcn.h section 11
+    _fields_ = [("width", ctypes.c_int32), ("height", ctypes.c_int32), ("x", ctypes.c_int32), ("y", ctypes.c_int32),
+                ("zoom", ctypes.c_double), ("mip_level", ctypes.c_int32), ("channels", ctypes.c_uint32), ("matte", ctypes.c_uint32)]
+
+
+VIEW_RED, VIEW_GREEN, VIEW_BLUE, VIEW_ALPHA = 0x4, 0x8, 0x10, 0x20
 
 
 class ShardPlan(ctypes.Structure):            # include/itw_bcn.h section 7
@@ -455,6 +463,56 @@ class ItwBcn(EncoderApi):
         if rc != 0:
             raise RuntimeError("itw_preview_pixels failed")
         return n.value
+
+    def preview_layers(self, dxgi_format, composite, layer0, flags=0, settings=None):
+        """itw_preview_layers: `composite` = host numpy H x W x planes array, `layer0` = (channels, alpha) as dds_encode_layers takes
+        one layer -> (display image, compressed bytes).  The display is float32 for BC6H at depth 32, uint8 otherwise."""
+        comp = np.ascontiguousarray(composite)
+        h, w = comp.shape[:2]
+        keep = []
+        arr = (LayerSource * 1)()
+        channels, alpha = layer0
+        planes = [np.ascontiguousarray(c, comp.dtype) for c in channels]
+        a = None if alpha is None else np.ascontiguousarray(alpha, comp.dtype)
+        keep += planes + [a]
+        arr[0].channel_count = len(planes)
+        for c, pl in enumerate(planes):
+            arr[0].channels[c] = pl.ctypes.data
+        arr[0].alpha = None if a is None else a.ctypes.data
+        img = np.zeros((h, w, 4), np.float32 if (dxgi_format in (95, 96) and comp.itemsize == 4) else np.uint8)
+        src = PixelSource(comp.ctypes.data, w, h, comp.shape[2], comp.itemsize * 8, 0)
+        sp = ctypes.cast(ctypes.byref(settings), ctypes.c_void_p) if settings is not None else None
+        size = ctypes.c_size_t(0)
+        rc = self.preview_layers_raw(dxgi_format, src, arr, flags, sp, RgbaSurface(img.ctypes.data, w, h, img.strides[0]), ctypes.byref(size))
+        if rc != 0:
+            raise RuntimeError("itw_preview_layers failed: " + self.last_error())
+        return img, size.value
+
+    def preview_layers_raw(self, dxgi_format, composite, layer0, flags, settings_ptr, display, size_ref):
+        """itw_preview_layers on ctypes structures; returns its status."""
+        f = self.lib.itw_preview_layers
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.c_int, ctypes.POINTER(PixelSource), ctypes.POINTER(LayerSource), ctypes.c_uint32, ctypes.c_void_p,
+                      ctypes.POINTER(RgbaSurface), ctypes.POINTER(ctypes.c_size_t)]
+        return f(dxgi_format, ctypes.byref(composite), layer0, flags, settings_ptr, ctypes.byref(display), size_ref)
+
+    def preview_view(self, source, view):
+        """itw_preview_view: `source` = host numpy H x W x planes array (uint8 depth 8, uint16 depth 16, float32 depth 32: the
+        document, or a pane of itw_preview_pixels), `view` = a View -> the view->height x view->width x 3 uint8 dialog buffer."""
+        src = np.ascontiguousarray(source)
+        out = np.zeros((view.height, view.width, 3), np.uint8)
+        ps = PixelSource(src.ctypes.data, src.shape[1], src.shape[0], src.shape[2], src.itemsize * 8, 0)
+        if self.preview_view_raw(ps, view, out.ctypes.data) != 0:
+            raise RuntimeError("itw_preview_view failed: " + self.last_error())
+        return out
+
+    def preview_view_raw(self, source, view, dst_ptr):
+        """itw_preview_view on ctypes structures and a raw (host or device) address; returns its status."""
+        f = self.lib.itw_preview_view
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.POINTER(PixelSource), ctypes.POINTER(View), ctypes.c_void_p]
+        return f(ctypes.byref(source) if source is not None else None, ctypes.byref(view) if view is not None else None,
+                 ctypes.c_void_p(dst_ptr) if dst_ptr else None)
 
     def dds_open(self, file_ptr, size):
         """itw_dds_open on a raw address (host or device): header + alpha check -> DdsOpenInfo."""

@@ -28,6 +28,7 @@
 #include "display.cuh"
 #include "open.cuh"
 #include "frontend.cuh"
+#include "view.cuh"
 #include "mips_f16.cuh"
 #include "itw_params.h"
 
