@@ -564,6 +564,42 @@ typedef struct itw_view {
  * 0..30, channel bits other than ITW_VIEW_*): `dst` is then untouched.  Returns 0 on success. */
 int itw_preview_view(const itw_pixel_source* source, const itw_view* view, uint8_t* dst);
 
+/* GetUncompressedImageForPreview (IntelPlugin.cpp:1085-1167): the original pane when the mip-map type is FROM_LAYERS or the texture
+ * type is a cube type (FetchPreviewRGB, :565-580), and the compressed pane of the "none" encoding, which the dialog takes from this
+ * function because GetCompressedImageForPreview returns NULL for it (:936-941, :551-552).  Every encoding but BC6H_UF16 gives an
+ * R8G8B8A8_UNORM scratch, so the pane is built in the plug-in's order with no DirectX::Convert:
+ *   CopyDataForEncoding(DoMipMaps = false, gammaCorrect = false): the ConvertToBC4or5From* front end for 80 / 83, ConvertToBCFrom*
+ *       for every other encoding (28 included); no _SRGB scratch, and depth 32 WITHOUT the v^(1/2.2) step
+ *   cube types (:1105-1121): the faces as itw_preview_cube builds them (never linearised), the chain to L when set, and the zeroed
+ *       horizontal cross of level L (4 wL x 3 hL).  A cross without L is the converted document, as for ITW_PANE_2D
+ *   mip maps from layers: layer 0 over the converted document (CopyLayersIntoMipMaps(..., 0, 1)) with the per-texel rules of
+ *       itw_dds_encode_layers: white alpha when the layer has none (15360 at depth 16) and the v^(1/2.2) step for 32-bit layers
+ *   FlipXYChannelNormalMap (:1137-1140), after layer 0
+ * and nothing else: no normalisation, padding, encode or decode.  The pane depends on the encoding only through its front end, so
+ * 28, 71, 72, 77, 78, 98 and 99 give one pane. */
+enum { ITW_PANE_2D = 0, ITW_PANE_CUBE_CROSS = 1, ITW_PANE_CUBE_LAYERS = 2 };
+typedef struct itw_pane_options {
+    uint32_t dxgi_format;  /* the dialog's encoding: 71/72 BC1, 77/78 BC3, 80 BC4, 83 BC5, 98/99 BC7 or 28 (none, R8G8B8A8_UNORM).
+                              95 is refused (its pane goes through WIC), 96 and every other id too                               */
+    int32_t  texture;      /* ITW_PANE_2D (COLOR, COLOR+A, NORMAL MAP) or one of the two cube types                            */
+    int32_t  mip_level;    /* cube types: the set mip level (SetMipLevel ? MipLevel : -1), -1 <= L < max(W, H).bit_length() of
+                              the face; ITW_PANE_2D: must be -1                                                                  */
+} itw_pane_options;
+/* The pane into `display` (R8G8B8A8_UNORM: 4-byte texels, rows `stride` >= 4 * width bytes apart).  `display` has the size of the
+ * document (ITW_PANE_2D, or a cross without L) or of the cross of level L.  A device display that is 4-byte aligned (pointer and
+ * stride) is written in place, so itw_preview_view can sample it with no copy; a host display receives one device-to-host copy.
+ * `layers`: ITW_PANE_2D: NULL, or layer 0 when the host's IsMipMapsDefinedByLayer() holds (read whole, document-sized planes of the
+ * document's depth); ITW_PANE_CUBE_LAYERS: six faces +X,-X,+Y,-Y,+Z,-Z as for itw_dds_encode_cube (channels[0] NULL for a face
+ * without a layer); ITW_PANE_CUBE_CROSS: ignored.  `flags`: ITW_FRONT_HAS_ALPHA (the plug-in's planes > 3), and ITW_FRONT_FLIP_X /
+ * _Y for ITW_PANE_2D only; ITW_FRONT_GAMMA and ITW_FRONT_NORMALIZE are refused (the pane never takes either step).
+ * *compressed_bytes (may be NULL) receives the dialog's compressed size: width * height * 4 of the DOCUMENT for 28 (also for the
+ * cube types, whose pane is the larger cross, :939), 0 for the other encodings.  Every operand may be host or device memory (device
+ * operands: the ordering rule of CompressBlocks*); synchronous; itw_last_kernel_ms gives the time of the call's kernels.  Every
+ * argument is checked before anything is enqueued (those itw_preview_layers and itw_preview_cube check, the encoding, BC4 / BC5 with
+ * a cube type, flags, a set level for ITW_PANE_2D): `display` is then untouched.  Returns 0 on success. */
+int itw_preview_uncompressed(const itw_pane_options* o, const itw_pixel_source* document, const itw_layer_source* layers,
+                             uint32_t flags, const rgba_surface* display, size_t* compressed_bytes);
+
 #ifdef __cplusplus
 }
 #endif

@@ -52,7 +52,8 @@ EXPORTS = (["CompressBlocksBC1", "CompressBlocksBC3", "CompressBlocksBC4", "Comp
             "CompressImageMT", "CompressImageST", "CompressImageBC1", "CompressImageBC3",
             "itw_shard_plan_make", "itw_shard_unique_id", "itw_shard_init", "itw_shard_finalize", "itw_encode_mip_chain_sharded",
             "itw_decompress", "itw_preview_pixels", "itw_dds_open", "itw_dds_open_layout", "itw_dds_read_layer",
-            "itw_dds_encode_layers", "itw_cube_layout", "itw_dds_encode_cube", "itw_preview_cube", "itw_preview_layers", "itw_preview_view"]
+            "itw_dds_encode_layers", "itw_cube_layout", "itw_dds_encode_cube", "itw_preview_cube", "itw_preview_layers", "itw_preview_view",
+            "itw_preview_uncompressed"]
            + ["CompressImageBC7_" + p for p in BC7_PROFILES] + ["CompressImage" + p.replace("bc6h_", "BC6H_") for p in BC6H_PROFILES]
            + ["GetProfile_" + p for p in BC7_PROFILES + BC6H_PROFILES])
 
@@ -97,6 +98,13 @@ class View(ctypes.Structure):                 # include/itw_bcn.h section 11
 
 
 VIEW_RED, VIEW_GREEN, VIEW_BLUE, VIEW_ALPHA = 0x4, 0x8, 0x10, 0x20
+
+
+class PaneOptions(ctypes.Structure):          # include/itw_bcn.h section 11
+    _fields_ = [("dxgi_format", ctypes.c_uint32), ("texture", ctypes.c_int32), ("mip_level", ctypes.c_int32)]
+
+
+PANE_2D, PANE_CUBE_CROSS, PANE_CUBE_LAYERS = 0, 1, 2
 
 
 class ShardPlan(ctypes.Structure):            # include/itw_bcn.h section 7
@@ -513,6 +521,38 @@ class ItwBcn(EncoderApi):
         f.argtypes = [ctypes.POINTER(PixelSource), ctypes.POINTER(View), ctypes.c_void_p]
         return f(ctypes.byref(source) if source is not None else None, ctypes.byref(view) if view is not None else None,
                  ctypes.c_void_p(dst_ptr) if dst_ptr else None)
+
+    def preview_uncompressed(self, options, document, layers=None, flags=0):
+        """itw_preview_uncompressed on host arrays -> (uint8 H x W x 4 pane, compressed bytes).  `document` = host numpy H x W x planes
+        array; `layers` = None, or for PANE_2D one layer (channels, alpha) and for PANE_CUBE_LAYERS six entries as cube_faces takes
+        them.  The pane is the document's size (2-D, or a cross without a set level) or the 4 wL x 3 hL cross of level L."""
+        doc = np.ascontiguousarray(document)
+        dh, dw = doc.shape[:2]
+        w, h = dw, dh
+        if options.texture != PANE_2D and not (options.texture == PANE_CUBE_CROSS and options.mip_level < 0):
+            fw, fh = (dw, dh) if options.texture == PANE_CUBE_LAYERS else ((dw // 3, dh // 4) if dw < dh else (dw // 4, dh // 3))
+            L = max(options.mip_level, 0)
+            w, h = 4 * max(1, fw >> L), 3 * max(1, fh >> L)
+        keep = []
+        arr = None
+        if layers is not None:
+            arr = self.cube_faces([layers] if options.texture == PANE_2D else layers, doc.dtype, keep)
+        img = np.zeros((h, w, 4), np.uint8)
+        src = PixelSource(doc.ctypes.data, dw, dh, doc.shape[2], doc.itemsize * 8, 0)
+        size = ctypes.c_size_t(0)
+        rc = self.preview_uncompressed_raw(options, src, arr, flags, RgbaSurface(img.ctypes.data, w, h, img.strides[0]), ctypes.byref(size))
+        if rc != 0:
+            raise RuntimeError("itw_preview_uncompressed failed: " + self.last_error())
+        return img, size.value
+
+    def preview_uncompressed_raw(self, options, document, layers, flags, display, size_ref):
+        """itw_preview_uncompressed on ctypes structures (any of them may be None); returns its status."""
+        f = self.lib.itw_preview_uncompressed
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.POINTER(PaneOptions), ctypes.POINTER(PixelSource), ctypes.POINTER(LayerSource), ctypes.c_uint32,
+                      ctypes.POINTER(RgbaSurface), ctypes.POINTER(ctypes.c_size_t)]
+        ref = lambda x: ctypes.byref(x) if x is not None else None
+        return f(ref(options), ref(document), layers, flags, ref(display), size_ref)
 
     def dds_open(self, file_ptr, size):
         """itw_dds_open on a raw address (host or device): header + alpha check -> DdsOpenInfo."""
