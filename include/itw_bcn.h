@@ -600,6 +600,43 @@ typedef struct itw_pane_options {
 int itw_preview_uncompressed(const itw_pane_options* o, const itw_pixel_source* document, const itw_layer_source* layers,
                              uint32_t flags, const rgba_surface* display, size_t* compressed_bytes);
 
+/* ---------------------------------------------------------------------------------------------
+ * Section 12 -- saving the "none" encoding: the uncompressed R8G8B8A8_UNORM (DXGI 28) DDS file that DoWriteDDS writes when the
+ * dialog's encoding is "none" (IntelPlugin.cpp:2051-2194), for every texture type the dialog allows it with (COLOR, COLOR+A, NORMAL
+ * MAP and both cube types, IsCombinationValid :44-65).  The steps are those of the other saves, in the plug-in's order:
+ *   CopyDataForEncoding(DoMipMaps, gammaCorrect = true): the ConvertToBCFrom* front end (:147-177), the v^(1/2.2) step at depth 32
+ *       with ITW_FRONT_GAMMA; the scratch is always R8G8B8A8_UNORM (28 is not sRGB, so there is no _SRGB scratch)
+ *   cube types: the faces of itw_dds_encode_cube (never linearised), the chain to L with a set level
+ *   2-D: layer 0 over level 0 (mip maps from layers), FlipXYChannelNormalMap, the chain, layers 1.. into their levels,
+ *       NormalizeNormalMapChain on every level
+ * and then no encode (CompressToScratchImage swaps the scratch in, :262-268): SaveToDDSMemory (or SaveCubeMipLevelToDDSFile, :1856-1871,
+ * for a set level) writes every level as it is, rows of 4 * w_l bytes with no padding, item-major and mip-minor, behind the legacy
+ * 128-byte header of _EncodeDDSHeader (DDSPF_A8B8G8R8, DDS_HEADER_FLAGS_PITCH, pitch 4 * width; one cube of six faces stays legacy).
+ * The chain is DirectXTex's non-WIC generators (box for power-of-two sizes, else linear), as for every UNORM save here; the plug-in's
+ * GenerateMipMaps hands R8G8B8A8_UNORM to WIC, which is not in the tree, so parity with WIC's filters is not pinned.
+ * Format 28 stays unknown to every other call of this header (itw_dds_header_bytes, itw_dds_write_header, itw_dds_open, ...).
+ * ------------------------------------------------------------------------------------------- */
+typedef struct itw_none_options {
+    int32_t texture;       /* ITW_PANE_2D (COLOR, COLOR+A, NORMAL MAP), ITW_PANE_CUBE_CROSS or ITW_PANE_CUBE_LAYERS                    */
+    int32_t mip_maps;      /* 0 / 1: the dialog's DoMipMaps (mip-map type AUTOGEN or FROM_LAYERS)                                     */
+    int32_t mip_level;     /* cube types: -1, or the set mip level L with the bound of itw_cube_layout; ITW_PANE_2D: must be -1         */
+} itw_none_options;
+/* Pure arithmetic, no CUDA call: the desc of the file (dxgi_format 28) and the level-0 size of an item (*face_width / *face_height:
+ * the document for ITW_PANE_2D, the face for the cube types; each may be NULL).  ITW_PANE_2D: the document, the full chain
+ * (max(W, H).bit_length() levels) with mip_maps, else one level.  Cube types: as itw_cube_layout.  Returns the file size, 128 +
+ * the sum over items and levels of 4 * w_l * h_l; 0 with an error text when refused. */
+size_t itw_dds_none_layout(const itw_none_options* o, int doc_width, int doc_height, itw_dds_desc* desc, int* face_width, int* face_height);
+/* DoWriteDDS with the "none" encoding into `file` (capacity >= the size itw_dds_none_layout gives).
+ * ITW_PANE_2D: `document` is the composite; `layers` / `layer_count` as for itw_dds_encode_layers (layer_count 0 when the host's
+ * IsMipMapsDefinedByLayer() is false); every ITW_FRONT_* flag applies.  Cube types: `document` and `layers` (the six faces, layer_count
+ * 6; ignored for a cross) as for itw_dds_encode_cube; only ITW_FRONT_HAS_ALPHA and ITW_FRONT_GAMMA apply.  Every operand may be host
+ * or device memory (device operands: the ordering rule of CompressBlocks*); synchronous; itw_last_kernel_ms gives the time of the
+ * call's kernels.  Every argument is checked before anything is enqueued (those of itw_dds_encode_layers and itw_dds_encode_cube,
+ * the options, layer_count, the file and its capacity): `file` is then untouched.  Returns the file size, or 0 with an error text
+ * that starts with the call's name. */
+size_t itw_dds_save_none(const itw_none_options* o, const itw_pixel_source* document, const itw_layer_source* layers, int layer_count,
+                         uint32_t flags, uint8_t* file, size_t capacity);
+
 #ifdef __cplusplus
 }
 #endif

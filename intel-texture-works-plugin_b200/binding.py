@@ -53,7 +53,7 @@ EXPORTS = (["CompressBlocksBC1", "CompressBlocksBC3", "CompressBlocksBC4", "Comp
             "itw_shard_plan_make", "itw_shard_unique_id", "itw_shard_init", "itw_shard_finalize", "itw_encode_mip_chain_sharded",
             "itw_decompress", "itw_preview_pixels", "itw_dds_open", "itw_dds_open_layout", "itw_dds_read_layer",
             "itw_dds_encode_layers", "itw_cube_layout", "itw_dds_encode_cube", "itw_preview_cube", "itw_preview_layers", "itw_preview_view",
-            "itw_preview_uncompressed"]
+            "itw_preview_uncompressed", "itw_dds_none_layout", "itw_dds_save_none"]
            + ["CompressImageBC7_" + p for p in BC7_PROFILES] + ["CompressImage" + p.replace("bc6h_", "BC6H_") for p in BC6H_PROFILES]
            + ["GetProfile_" + p for p in BC7_PROFILES + BC6H_PROFILES])
 
@@ -105,6 +105,10 @@ class PaneOptions(ctypes.Structure):          # include/itw_bcn.h section 11
 
 
 PANE_2D, PANE_CUBE_CROSS, PANE_CUBE_LAYERS = 0, 1, 2
+
+
+class NoneOptions(ctypes.Structure):          # include/itw_bcn.h section 12
+    _fields_ = [("texture", ctypes.c_int32), ("mip_maps", ctypes.c_int32), ("mip_level", ctypes.c_int32)]
 
 
 class ShardPlan(ctypes.Structure):            # include/itw_bcn.h section 7
@@ -553,6 +557,48 @@ class ItwBcn(EncoderApi):
                       ctypes.POINTER(RgbaSurface), ctypes.POINTER(ctypes.c_size_t)]
         ref = lambda x: ctypes.byref(x) if x is not None else None
         return f(ref(options), ref(document), layers, flags, ref(display), size_ref)
+
+    def none_layout(self, options, doc_width, doc_height):
+        """itw_dds_none_layout: (file size, DdsDesc, level-0 width, level-0 height); size 0 (and the error text) when refused."""
+        f = self.lib.itw_dds_none_layout
+        f.restype = ctypes.c_size_t
+        f.argtypes = [ctypes.POINTER(NoneOptions), ctypes.c_int, ctypes.c_int, ctypes.POINTER(DdsDesc), ctypes.POINTER(ctypes.c_int),
+                      ctypes.POINTER(ctypes.c_int)]
+        d, fw, fh = DdsDesc(), ctypes.c_int(0), ctypes.c_int(0)
+        n = f(ctypes.byref(options) if options is not None else None, doc_width, doc_height, ctypes.byref(d), ctypes.byref(fw), ctypes.byref(fh))
+        return n, d, fw.value, fh.value
+
+    def dds_save_none(self, options, document, layers=None, flags=0):
+        """itw_dds_save_none on host arrays -> the file (uint8).  `document` = host numpy H x W x planes array; `layers` = ITW_PANE_2D:
+        None or a list of (channels, alpha) as dds_encode_layers takes them; ITW_PANE_CUBE_LAYERS: six entries as cube_faces takes them;
+        ignored for a cross."""
+        doc = np.ascontiguousarray(document)
+        n = self.none_layout(options, doc.shape[1], doc.shape[0])[0]
+        if not n:
+            raise ValueError("itw_dds_none_layout refused the options: " + self.last_error())
+        keep, arr, count = [], None, 0
+        if options.texture == PANE_CUBE_LAYERS:
+            arr, count = self.cube_faces(layers, doc.dtype, keep), 6
+        elif options.texture == PANE_2D and layers:
+            arr, count = (LayerSource * len(layers))(), len(layers)
+            for i, (channels, alpha) in enumerate(layers):
+                one = self.cube_faces([(channels, alpha)], doc.dtype, keep)
+                arr[i] = one[0]
+        src = PixelSource(doc.ctypes.data, doc.shape[1], doc.shape[0], doc.shape[2], doc.itemsize * 8, 0)
+        out = np.zeros(n, np.uint8)
+        got = self.dds_save_none_raw(options, src, arr, count, flags, out.ctypes.data, n)
+        if got != n:
+            raise RuntimeError("itw_dds_save_none failed: " + self.last_error())
+        return out
+
+    def dds_save_none_raw(self, options, document, layers, count, flags, file_ptr, capacity):
+        """itw_dds_save_none on ctypes structures (options and document may be None) and raw addresses; returns the file size (0 on error)."""
+        f = self.lib.itw_dds_save_none
+        f.restype = ctypes.c_size_t
+        f.argtypes = [ctypes.POINTER(NoneOptions), ctypes.POINTER(PixelSource), ctypes.POINTER(LayerSource), ctypes.c_int, ctypes.c_uint32,
+                      ctypes.c_void_p, ctypes.c_size_t]
+        ref = lambda x: ctypes.byref(x) if x is not None else None
+        return f(ref(options), ref(document), layers, count, flags, ctypes.c_void_p(file_ptr) if file_ptr else None, capacity)
 
     def dds_open(self, file_ptr, size):
         """itw_dds_open on a raw address (host or device): header + alpha check -> DdsOpenInfo."""

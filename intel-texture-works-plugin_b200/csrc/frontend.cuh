@@ -137,6 +137,13 @@ ITW_HD void front_normalize_hdr(u32& r, u32& g, u32& b)
         b = front_half_from_float(fb * m);
     } else { r = 0u; g = 0u; b = 0x3C00u; }
 }
+// the same on one stored RGBA8 texel: r, g and b normalised, alpha kept (normalize_kernel and none_store_kernel)
+ITW_HD u32 front_normalize_rgba8(u32 v)
+{
+    u32 r = v & 255u, g = (v >> 8) & 255u, b = (v >> 16) & 255u;
+    front_normalize_ldr(r, g, b);
+    return r | (g << 8) | (b << 16) | (v & 0xFF000000u);
+}
 
 // FlipXYChannelNormalMap on one texel: IP:1519-1527 (bytes) and IP:1531-1542 (halves)
 ITW_HD void front_flip_ldr(u32& r, u32& g, u32 flags)
@@ -303,10 +310,7 @@ __global__ void __launch_bounds__(256) normalize_kernel(uint8_t* __restrict__ pt
         p[1] = b | (a << 16);
     } else {
         u32* p = reinterpret_cast<u32*>(ptr + (long long)y * stride + (long long)x * 4);
-        const u32 v = *p;
-        u32 r = v & 255u, g = (v >> 8) & 255u, b = (v >> 16) & 255u;
-        front_normalize_ldr(r, g, b);
-        *p = r | (g << 8) | (b << 16) | (v & 0xFF000000u);
+        *p = front_normalize_rgba8(*p);
     }
 }
 // Layers into mip levels: every level of `P` in ONE launch, one thread per written texel, the levels back to back in the

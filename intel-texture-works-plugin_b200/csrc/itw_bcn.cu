@@ -28,6 +28,7 @@
 #include "display.cuh"
 #include "open.cuh"
 #include "frontend.cuh"
+#include "none.cuh"
 #include "view.cuh"
 #include "mips_f16.cuh"
 #include "itw_params.h"
@@ -1100,3 +1101,4 @@ int itw_bc7_phase_clocks(void* out, size_t bytes)
 #include "itw_preview.inc"
 #include "itw_open.inc"
 #include "itw_cube.inc"
+#include "itw_none.inc"
