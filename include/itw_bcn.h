@@ -441,7 +441,7 @@ int itw_preview_pixels(int dxgi_format, const itw_pixel_source* sources, int cou
  *                                               to R8G8B8A8_UNORM[_SRGB] or R32G32B32A32_FLOAT
  *   DoReadContinue (IntelPlugin.cpp:2614-2742)  once per layer: zero a full-size interleaved buffer, copy one image into it
  * The formats are those of itw_dds_desc: BC1, BC3, BC4, BC5, BC6H UF16 / SF16, BC7 and the _SRGB forms.  BC2, uncompressed and
- * palettised files are rejected.
+ * palettised files are rejected (section 13 opens the uncompressed files the plug-in reads without a conversion).
  * ------------------------------------------------------------------------------------------- */
 typedef struct itw_dds_open_info {
     itw_dds_desc desc;        /* as itw_dds_read_header                                                                */
@@ -614,7 +614,8 @@ int itw_preview_uncompressed(const itw_pane_options* o, const itw_pixel_source* 
  * 128-byte header of _EncodeDDSHeader (DDSPF_A8B8G8R8, DDS_HEADER_FLAGS_PITCH, pitch 4 * width; one cube of six faces stays legacy).
  * The chain is DirectXTex's non-WIC generators (box for power-of-two sizes, else linear), as for every UNORM save here; the plug-in's
  * GenerateMipMaps hands R8G8B8A8_UNORM to WIC, which is not in the tree, so parity with WIC's filters is not pinned.
- * Format 28 stays unknown to every other call of this header (itw_dds_header_bytes, itw_dds_write_header, itw_dds_open, ...).
+ * Format 28 stays unknown to every other call of this header (itw_dds_header_bytes, itw_dds_write_header, itw_dds_open, ...); section 13
+ * opens these files.
  * ------------------------------------------------------------------------------------------- */
 typedef struct itw_none_options {
     int32_t texture;       /* ITW_PANE_2D (COLOR, COLOR+A, NORMAL MAP), ITW_PANE_CUBE_CROSS or ITW_PANE_CUBE_LAYERS                    */
@@ -636,6 +637,60 @@ size_t itw_dds_none_layout(const itw_none_options* o, int doc_width, int doc_hei
  * that starts with the call's name. */
 size_t itw_dds_save_none(const itw_none_options* o, const itw_pixel_source* document, const itw_layer_source* layers, int layer_count,
                          uint32_t flags, uint8_t* file, size_t capacity);
+
+/* ---------------------------------------------------------------------------------------------
+ * Section 13 -- opening uncompressed files: the DDS files whose loaded format (LoadFromDDSMemory with DDS_FLAGS_NONE, the header
+ * rules of _DecodeDDSHeader / _GetDXGIFormat, DirectXTexDDS.cpp:144-437) is already DoReadStart's target (IntelPlugin.cpp:2534-2553),
+ * so the plug-in runs neither Decompress nor Convert:
+ *   28 R8G8B8A8_UNORM       -> depth 8        29 R8G8B8A8_UNORM_SRGB -> depth 8
+ *   11 R16G16B16A16_UNORM   -> depth 16       2 R32G32B32A32_FLOAT   -> depth 32
+ * The files of itw_dds_save_none are among them.  The header forms accepted (ITW_RAW_*) are a 'DX10' header naming 2, 11, 28 or 29,
+ * and the legacy pixel formats that load as one of them.  A legacy header is matched as _GetDXGIFormat matches it: the first entry
+ * of g_LegacyDDSMap whose flags intersect the header's and whose FourCC (FourCC entries), bit count (palette entries) or bit count
+ * and four masks (the others) are equal.  Refused, with a message naming the call and the reason: every file whose loaded format
+ * differs from its target (A8R8G8B8 / X8R8G8B8 load as B8G8R8A8 / B8G8R8X8, 565, 5551, 4444, L8, L16, A8L8, A8, G16R16, 10:10:10:2,
+ * FourCC 113 and the other float FourCCs, DX10 ids other than the four above: the plug-in converts them with DirectX::Convert, which
+ * can hand them to WIC), the palettised and 3:3:2 / 4:4 expansions (P8, A8P8, A8R3G3B2, R3G3B2, A4L4), block-compressed files (use
+ * itw_dds_open), volumes, arrays other than one cube map, partial cubes, truncated files, width or height 0 or above 16777216.
+ * The shapes are those of itw_dds_open: a 2-D texture with or without a mip chain, or one cube map (six faces).
+ * ------------------------------------------------------------------------------------------- */
+enum {
+    ITW_RAW_DX10 = 0,        /* 'DX10' extension header naming 2, 11, 28 or 29 (payload at 148)                                  */
+    ITW_RAW_A8B8G8R8 = 1,    /* DDSPF_A8B8G8R8 -> 28 (the header of itw_dds_save_none)                                           */
+    ITW_RAW_X8B8G8R8 = 2,    /* DDSPF_X8B8G8R8 -> 28 with alpha 255 (CONV_FLAGS_NOALPHA)                                         */
+    ITW_RAW_R8G8B8 = 3,      /* DDSPF_R8G8B8, 24 bpp -> 28: rows of 3 w bytes, texels stored B, G, R, alpha 255 (CONV_FLAGS_888)  */
+    ITW_RAW_A16B16G16R16 = 4,/* FourCC 36 -> 11                                                                                  */
+    ITW_RAW_A32B32G32R32F = 5/* FourCC 116 -> 2                                                                                  */
+};
+typedef struct itw_dds_uncompressed_info {
+    itw_dds_desc desc;        /* width, height, mip_levels, array_size (1 or 6), is_cubemap; dxgi_format = the loaded format:
+                                 2, 11, 28 or 29 (unknown to the calls of section 3, which keep refusing these formats)          */
+    int32_t source;           /* ITW_RAW_*: the header form                                                                     */
+    uint64_t payload_offset;  /* where the payload starts in the file: 128, or 148 behind a 'DX10' header                         */
+    int32_t has_alpha;        /* loadInfo.hasAlpha: !IsAlphaAllOpaque() over every texel of every image (alpha < 0.99f); always 0
+                                 for X8B8G8R8 and R8G8B8, whose alpha the loader sets to 255.  Taken before the cube-map override  */
+    int32_t has_mips, ask_user;   /* as in itw_dds_open_info                                                                     */
+    /* filled by itw_dds_uncompressed_layout, with the meanings of itw_dds_open_info: */
+    int32_t layers, calls, planes;
+    int32_t depth;            /* 8 (bytes), 16 (ushorts) or 32 (floats) bits per channel                                         */
+    int32_t width, height;
+    int32_t target_dxgi;      /* the loaded format, which is the target: 2, 11, 28 or 29                                         */
+} itw_dds_uncompressed_info;
+/* Header + the alpha check on the GPU.  Fills desc, source, payload_offset, has_alpha, has_mips and ask_user; zeroes the layout
+ * fields.  A device-resident file is scanned where it lies; a host file's payload is copied to the device once.  Synchronous;
+ * itw_last_kernel_ms gives the scan's time (-1 when the form needs no scan).  Returns 0 on success; on failure `info` is untouched. */
+int itw_dds_open_uncompressed(const uint8_t* file, size_t size, itw_dds_uncompressed_info* info);
+/* The layout for the dialog's answers `options` (ITW_OPEN_*), with itw_dds_open_layout's decisions; pure arithmetic, no CUDA call.
+ * Returns 0 on success. */
+int itw_dds_uncompressed_layout(itw_dds_uncompressed_info* info, uint32_t options);
+/* One DoReadContinue, with the image choice, the zeroed layer and the rules of itw_dds_read_layer: channels 0..planes-1 of the loaded
+ * texel (R8G8B8 and X8B8G8R8 expanded with alpha 255), and for a cube map with has_alpha the last plane forced to 255 (depth 8), 1.0f
+ * (depth 32) or 0x3C00 (depth 16: the plug-in's ConvertTo16Bit((unsigned8)255), a half-float 1.0 in a UNORM16 plane).  16-bit
+ * planes receive the file's 0..65535 values unscaled, as the plug-in hands them to Photoshop.  `file` and `dst` may each be host or
+ * device memory (device operands: the ordering rule of CompressBlocks*); synchronous.  Every argument is checked before anything is
+ * enqueued: on failure dst is untouched.  Returns 0 on success. */
+int itw_dds_read_uncompressed_layer(const uint8_t* file, size_t size, const itw_dds_uncompressed_info* info, int call, void* dst,
+                                    int64_t row_bytes);
 
 #ifdef __cplusplus
 }

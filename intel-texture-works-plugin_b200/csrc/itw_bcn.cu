@@ -11,6 +11,7 @@
 
 #include <atomic>
 #include <condition_variable>
+#include <cstdarg>
 #include <cstdio>
 #include <cstring>
 #include <functional>
@@ -27,6 +28,7 @@
 #include "decode.cuh"
 #include "display.cuh"
 #include "open.cuh"
+#include "open_raw.cuh"
 #include "frontend.cuh"
 #include "none.cuh"
 #include "view.cuh"
@@ -1100,5 +1102,6 @@ int itw_bc7_phase_clocks(void* out, size_t bytes)
 #include "itw_shard.inc"
 #include "itw_preview.inc"
 #include "itw_open.inc"
+#include "itw_open_raw.inc"
 #include "itw_cube.inc"
 #include "itw_none.inc"

@@ -22,7 +22,7 @@
 // the display decoders (display.cuh) unchanged; the rest of the layer is zeros, so every byte of the layer is written exactly once and
 // no memset pass precedes it.  Each lane packs its tile's row of texels (12, 16, 48 or 64 bytes) into the warp's row in shared memory;
 // the warp then stores that row with 16-byte stores (plus a byte tail at the layer's right edge), so three-plane rows leave as whole
-// 128-byte lines rather than as 12-byte pieces.
+// 128-byte lines rather than as 12-byte pieces (store_staged_row, which open_raw.cuh's layer kernel shares).
 #pragma once
 #include "display.cuh"
 
@@ -60,6 +60,42 @@ struct OpenImage {
 };
 
 #if defined(__CUDACC__)
+// The row-staged store shared by the open path's layer kernels.  A warp writes one stretch of a layer row: lane k supplies the k-th
+// kTileRow-byte piece of it (four texels), the pieces meet in shared memory, and the warp stores the first `span` bytes with 16-byte
+// stores plus a byte tail at the layer's right edge, so rows of 3-plane texels leave as whole 128-byte lines.  Pieces of 16, 32, 48
+// and 64 bytes go in as 16-byte stores (lanes 16 and 48 bytes apart meet 8 distinct bank quads per quarter warp); for 64 bytes one
+// spare 16-byte slot after every 128 bytes spreads the lanes of a quarter warp over all eight quads as well.  12- and 24-byte pieces
+// go in as words.  `srow` holds staged_row_slots(kTileRow) slots; dst and the row are 16-byte aligned.
+__host__ __device__ constexpr int staged_row_slots(int tile_row)
+{
+    return 2 * tile_row + (tile_row == 64 ? tile_row / 4 : 0);     // 32 pieces of 16-byte slots, plus the spare slots of 64-byte pieces
+}
+template <int kTileRow>
+__device__ __forceinline__ void store_staged_row(uint4* srow, int lane, bool has_piece, const u32 (&t)[kTileRow / 4], int span,
+                                                 uint8_t* grow)
+{
+    constexpr int kWords = kTileRow / 4;
+    constexpr int kVecs = kWords % 4 == 0 ? kWords / 4 : 0;
+    constexpr int kPad = kVecs == 4 ? 1 : 0;
+    auto slot = [](int k) { return k + kPad * (k >> 3); };      // smem slot of the row's k-th 16-byte piece
+    if (has_piece) {
+        if constexpr (kVecs > 0) {
+#pragma unroll
+            for (int j = 0; j < kVecs; j++) srow[slot(kVecs * lane + j)] = make_uint4(t[4 * j], t[4 * j + 1], t[4 * j + 2], t[4 * j + 3]);
+        } else {
+            u32* words = reinterpret_cast<u32*>(srow) + lane * kWords;
+#pragma unroll
+            for (int i = 0; i < kWords; i++) words[i] = t[i];
+        }
+    }
+    __syncwarp();
+    const int body = span & ~15;
+    for (int i = lane; i < body >> 4; i += 32) reinterpret_cast<uint4*>(grow)[i] = srow[slot(i)];
+    if (lane < span - body)
+        grow[body + lane] = reinterpret_cast<const uint8_t*>(srow + slot(body >> 4))[lane];
+    __syncwarp();
+}
+
 // One thread per block of every image; `images` sorted by `first`.  *flag becomes 1 if any texel of any image is not opaque.
 template <int kFormat>
 __global__ void __launch_bounds__(256) open_alpha_kernel(const uint8_t* __restrict__ payload, long long nblocks,
@@ -100,13 +136,7 @@ __global__ void __launch_bounds__(256, 2) open_layer_kernel(const uint8_t* __res
     constexpr int kTexel = kPlanes * (kHdr ? 4 : 1);            // bytes per layer texel
     constexpr int kTileRow = 4 * kTexel;                        // bytes of one tile's row: 12, 16, 48 or 64
     constexpr int kWords = kTileRow / 4;
-    // One layer row of 32 tiles per warp.  Tile rows of 16, 48 and 64 bytes go in as 16-byte stores (lanes 16 and 48 bytes apart
-    // meet 8 distinct bank quads per quarter warp); for 64 bytes one spare 16-byte slot after every 128 bytes (kPad) spreads the
-    // lanes of a quarter warp over all eight quads as well.  12-byte rows go in as words, 3 words apart: no conflict either.
-    constexpr int kVecs = kWords % 4 == 0 ? kWords / 4 : 0;
-    constexpr int kPad = kVecs == 4 ? 1 : 0;
-    constexpr int kSlots = 32 * kTileRow / 16;
-    __shared__ uint4 stage[8][kSlots + kPad * kSlots / 8];
+    __shared__ uint4 stage[8][staged_row_slots(kTileRow)];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int tw = (width + 3) >> 2, chunks = (tw + 31) >> 5;
     const long long g = (long long)blockIdx.x * 8 + warp;       // warp-uniform: (tile row, chunk of 32 tiles)
@@ -135,7 +165,6 @@ __global__ void __launch_bounds__(256, 2) open_layer_kernel(const uint8_t* __res
     const int span = min(128, width - 128 * chunk) * kTexel;    // bytes of the warp's part of a layer row
     uint8_t* out = dst + (long long)chunk * 128 * kTexel;
     uint4* srow = stage[warp];
-    auto slot = [](int k) { return k + kPad * (k >> 3); };      // smem slot of the row's k-th 16-byte piece
 #pragma unroll
     for (int y = 0; y < 4; y++) {
         const int Y = 4 * ty + y;
@@ -167,23 +196,7 @@ __global__ void __launch_bounds__(256, 2) open_layer_kernel(const uint8_t* __res
                 t[2] = ((q[2] >> 16) & 0xFFu) | (q[3] << 8);
             }
         }
-        if (tx < tw) {
-            if constexpr (kVecs > 0) {
-#pragma unroll
-                for (int j = 0; j < kVecs; j++) srow[slot(kVecs * lane + j)] = make_uint4(t[4 * j], t[4 * j + 1], t[4 * j + 2], t[4 * j + 3]);
-            } else {
-                u32* words = reinterpret_cast<u32*>(srow) + lane * kWords;
-#pragma unroll
-                for (int i = 0; i < kWords; i++) words[i] = t[i];
-            }
-        }
-        __syncwarp();
-        uint8_t* grow = out + (long long)Y * row_bytes;
-        const int body = span & ~15;
-        for (int i = lane; i < body >> 4; i += 32) reinterpret_cast<uint4*>(grow)[i] = srow[slot(i)];
-        if (lane < span - body)
-            grow[body + lane] = reinterpret_cast<const uint8_t*>(srow + slot(body >> 4))[lane];
-        __syncwarp();
+        store_staged_row<kTileRow>(srow, lane, tx < tw, t, span, out + (long long)Y * row_bytes);
     }
 }
 #endif
