@@ -153,7 +153,18 @@ int fail(const char* what, cudaError_t e = cudaSuccess)
     tls.err = buf;
     return -1;
 }
-#define ITW_CUDA(call)                                             \
+// fail() with "who: " and a formatted reason
+__attribute__((format(printf, 2, 3))) int fail_in(const char* who, const char* fmt, ...)
+{
+    char buf[320];
+    const int n = snprintf(buf, sizeof(buf), "%s: ", who);
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(buf + n, sizeof(buf) - n, fmt, ap);
+    va_end(ap);
+    return fail(buf);
+}
+#define ITW_CUDA(call)                                          \
     do {                                                           \
         cudaError_t e_ = (call);                                   \
         if (e_ != cudaSuccess) return fail(#call, e_);             \
@@ -771,6 +782,74 @@ int launch_front(const FrontParams& P, uint8_t* d_dst, int dw, int dh, long long
     ITW_CUDA(cudaGetLastError());
     return 0;
 }
+
+// The w x h surface at `src` padded to pw x ph tight rows at `dst` by edge replication (DoPaddingToMultiplesOf4).
+int launch_pad(const uint8_t* src, int w, int h, long long stride, int texel_bytes, uint8_t* dst, int pw, int ph, cudaStream_t s)
+{
+    const dim3 grid((unsigned)((pw + 63) / 64), (unsigned)ph);
+    if (texel_bytes == 8) pad_f16_kernel<<<grid, 64, 0, s>>>(src, w, h, stride, dst, pw, (long long)pw * 8);
+    else pad_rgba8_kernel<<<grid, 64, 0, s>>>(src, w, h, (int)stride, dst, pw, pw * 4);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail("pad kernel", e);
+}
+// Every texel of the w x h surface at `dst` set to (lo, hi); `words` 32-bit words per texel.
+int launch_fill(uint8_t* dst, int w, int h, long long stride, int words, u32 lo, u32 hi, cudaStream_t s)
+{
+    fill_texels_kernel<<<dim3((unsigned)((w + 255) / 256), (unsigned)h), 256, 0, s>>>(dst, w, h, stride, words, lo, hi);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail("fill_texels_kernel", e);
+}
+// NormalizeNormalMapChain's per-texel step over the w x h surface at `p`: RGBA16F when `hdr`, else RGBA8.
+int launch_normalize(uint8_t* p, int w, int h, long long stride, bool hdr, cudaStream_t s)
+{
+    normalize_kernel<<<dim3((unsigned)((w + 255) / 256), (unsigned)h), 256, 0, s>>>(p, w, h, stride, hdr ? 1 : 0);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail("normalize_kernel", e);
+}
+
+// ---- document layers (mip maps from layers, cube face layers, the layer-0 panes) ----
+// The planes of a layer that are read: colour planes 0..channel_count-1, and its alpha plane when the document has alpha.
+// Bytes of the lw x lh rectangle of `L` staged by stage_layer: one 16-byte aligned tight plane per plane read.
+size_t layer_stage_bytes(const itw_layer_source& L, int lw, int lh, int depth, bool alpha)
+{
+    const size_t plane = ((size_t)lw * lh * (depth / 8) + 15) & ~(size_t)15;
+    return plane * (size_t)(L.channel_count + (alpha && L.alpha ? 1 : 0));
+}
+// Copy the lw x lh top-left rectangle of every plane of `L` that is read (any memory; rows L.row_bytes apart, or one row of the
+// dw-texel document) to tight planes from `dst` on, and describe them in plane[], channels, lw and lh of `v`.  `dst` ends past them.
+int stage_layer(const itw_layer_source& L, int dw, int lw, int lh, int depth, bool alpha, uint8_t*& dst, LayerLevel& v, cudaStream_t s)
+{
+    const size_t row = (size_t)lw * (depth / 8), plane = (row * lh + 15) & ~(size_t)15;
+    const size_t pitch = L.row_bytes ? (size_t)L.row_bytes : (size_t)dw * (depth / 8);
+    v.lw = lw;
+    v.lh = lh;
+    v.channels = L.channel_count;
+    for (int p = 0; p < 4; p++) {
+        const void* src = p < L.channel_count ? L.channels[p] : (p == 3 && alpha ? L.alpha : nullptr);
+        if (!src) continue;
+        v.plane[p] = dst;
+        const cudaError_t e = cudaMemcpy2DAsync(dst, row, src, pitch, row, (size_t)lh, cudaMemcpyDefault, s);
+        if (e != cudaSuccess) return fail("layer H2D", e);
+        dst += plane;
+    }
+    return 0;
+}
+// Whether a plane of layers[0..n) that is read is device memory.  A layer whose channel 0 is null (a missing cube face) is not read.
+bool layers_on_device(const itw_layer_source* layers, int n, bool alpha)
+{
+    for (int i = 0; i < n; i++) {
+        const itw_layer_source& L = layers[i];
+        if (!L.channels[0]) continue;
+        for (int p = 0; p < L.channel_count; p++)
+            if (is_device_pointer(L.channels[p])) return true;
+        if (alpha && L.alpha && is_device_pointer(L.alpha)) return true;
+    }
+    return false;
+}
+
 int convert_any(int format, const itw_pixel_source* src, uint32_t flags, const rgba_surface* dst)
 {
     tls.err.clear();
