@@ -692,6 +692,59 @@ int itw_dds_uncompressed_layout(itw_dds_uncompressed_info* info, uint32_t option
 int itw_dds_read_uncompressed_layer(const uint8_t* file, size_t size, const itw_dds_uncompressed_info* info, int call, void* dst,
                                     int64_t row_bytes);
 
+/* ---------------------------------------------------------------------------------------------
+ * Section 14 -- opening converted files: the uncompressed DDS files whose loaded format DoReadStart converts with DirectX::Convert
+ * (IntelPlugin.cpp:2534-2560, filter 0) and for which _UseWICConversion (DirectXTexConvert.cpp:4161-4266) chooses the non-WIC _Convert:
+ * _LoadScanline, _ConvertScanline, _StoreScanline per texel.  Loaded format -> target / depth:
+ *   10 R16G16B16A16_FLOAT, 54 R16_FLOAT, 34 R16G16_FLOAT, 13 R16G16B16A16_SNORM, 35 R16G16_UNORM, 37 R16G16_SNORM, 58 R16_SNORM,
+ *   26 R11G11B10_FLOAT, 67 R9G9B9E5_SHAREDEXP                              -> 11 R16G16B16A16_UNORM, depth 16
+ *   49 R8G8_UNORM, 51 R8G8_SNORM, 31 R8G8B8A8_SNORM, 63 R8_SNORM, 65 A8_UNORM, 115 B4G4R4A4_UNORM -> 28 R8G8B8A8_UNORM, depth 8
+ *   16 R32G32_FLOAT                                                        -> 2 R32G32B32A32_FLOAT, depth 32
+ * SNORM channels become v * 0.5 + 0.5, FLOAT channels are saturated into UNORM targets, absent channels are 0 (alpha 1), and the
+ * one-channel formats R16_FLOAT, R16_SNORM and R8_SNORM are replicated into red, green and blue.  A8L8 loads as R8G8 (L in red, A in
+ * green, as DirectXTex loads it).  Refused, each with a message naming the call: the files Convert hands to WIC (A8R8G8B8 / X8R8G8B8
+ * and the other B8G8R8A8 / B8G8R8X8 forms, 565, 5551, 10:10:10:2, XR_BIAS, L8, L16, R32F, D32_FLOAT, D16_UNORM), R32G32B32_FLOAT
+ * (whose WIC use depends on the runtime), the four formats of section 13 (use itw_dds_open_uncompressed), block-compressed files (use
+ * itw_dds_open), UINT / SINT / typeless / other depth / video formats, RGBG / GRGB / YUY2 / UYVY, the palettised and 3:3:2 / 4:4 expansions, volumes, arrays other
+ * than one cube map, partial cubes and truncated files.  Shapes and rules are those of section 13.
+ * ------------------------------------------------------------------------------------------- */
+enum {
+    ITW_CONV_DX10 = 0,            /* 'DX10' extension header naming one of the loaded formats above (payload at 148)               */
+    ITW_CONV_G16R16 = 1,          /* D3DFMT_G16R16 -> 35                                                                          */
+    ITW_CONV_A8L8 = 2,            /* D3DFMT_A8L8 -> 49                                                                            */
+    ITW_CONV_A8 = 3,              /* D3DFMT_A8 -> 65                                                                              */
+    ITW_CONV_A4R4G4B4 = 4,        /* D3DFMT_A4R4G4B4 -> 115                                                                       */
+    ITW_CONV_X4R4G4B4 = 5,        /* D3DFMT_X4R4G4B4 -> 115 with the alpha nibble set to 0xF (CONV_FLAGS_NOALPHA)                  */
+    ITW_CONV_Q16W16V16U16 = 6,    /* FourCC 110 -> 13                                                                             */
+    ITW_CONV_R16F = 7,            /* FourCC 111 -> 54                                                                             */
+    ITW_CONV_G16R16F = 8,         /* FourCC 112 -> 34                                                                             */
+    ITW_CONV_A16B16G16R16F = 9,   /* FourCC 113 -> 10                                                                             */
+    ITW_CONV_G32R32F = 10         /* FourCC 115 -> 16                                                                             */
+};
+typedef struct itw_dds_converted_info {
+    itw_dds_desc desc;        /* width, height, mip_levels, array_size (1 or 6), is_cubemap; dxgi_format = the loaded format       */
+    int32_t form;             /* ITW_CONV_*: the header form                                                                    */
+    uint64_t payload_offset;  /* where the payload starts in the file: 128, or 148 behind a 'DX10' header                         */
+    int32_t has_alpha;        /* loadInfo.hasAlpha: HasAlpha(loaded) && !IsAlphaAllOpaque() (alpha < 0.99f, read as the loaded
+                                 format); always 0 for the formats without alpha and for X4R4G4B4.  Taken before the cube override */
+    int32_t has_mips, ask_user;   /* as in itw_dds_open_info                                                                     */
+    /* filled by itw_dds_converted_layout, with the meanings of itw_dds_open_info: */
+    int32_t layers, calls, planes;
+    int32_t depth;            /* 8 (bytes), 16 (ushorts) or 32 (floats) bits per channel                                         */
+    int32_t width, height;
+    int32_t target_dxgi;      /* the target: 2, 11 or 28                                                                         */
+} itw_dds_converted_info;
+/* Header + the alpha check on the GPU, as itw_dds_open_uncompressed.  itw_last_kernel_ms gives the scan's time (-1 when the format has
+ * no alpha).  Returns 0 on success; on failure `info` is untouched. */
+int itw_dds_open_converted(const uint8_t* file, size_t size, itw_dds_converted_info* info);
+/* The layout for the dialog's answers `options` (ITW_OPEN_*); pure arithmetic, no CUDA call.  Returns 0 on success. */
+int itw_dds_converted_layout(itw_dds_converted_info* info, uint32_t options);
+/* One DoReadContinue: the image the call reads, converted texel by texel into the target and stored into the zeroed layer, with the
+ * rules of itw_dds_read_uncompressed_layer (cube alpha forcing, 16-bit planes unscaled, host or device operands, every argument
+ * checked before anything is enqueued).  Returns 0 on success. */
+int itw_dds_read_converted_layer(const uint8_t* file, size_t size, const itw_dds_converted_info* info, int call, void* dst,
+                                 int64_t row_bytes);
+
 #ifdef __cplusplus
 }
 #endif

@@ -30,12 +30,65 @@ enum RawSource : int {
     kRawRgbx8 = 1,      // X8B8G8R8: R8G8B8A8_UNORM with alpha set to 255
     kRawBgr8 = 2,       // R8G8B8 (24 bpp): B, G, R bytes expanded to R8G8B8A8_UNORM with alpha 255
     kRawRgba16 = 3,     // R16G16B16A16_UNORM, copied
-    kRawRgba32f = 4     // R32G32B32A32_FLOAT, copied
+    kRawRgba32f = 4,    // R32G32B32A32_FLOAT, copied
+    // The converted forms (itw_open_conv.inc): the loaded format, put through DirectX::Convert's _Convert into the target
+    kConvRgba16f = 5,   // R16G16B16A16_FLOAT (10)        -> R16G16B16A16_UNORM
+    kConvR16f = 6,      // R16_FLOAT (54)                 -> R16G16B16A16_UNORM
+    kConvRg16f = 7,     // R16G16_FLOAT (34)              -> R16G16B16A16_UNORM
+    kConvRgba16s = 8,   // R16G16B16A16_SNORM (13)        -> R16G16B16A16_UNORM
+    kConvRg16 = 9,      // R16G16_UNORM (35)              -> R16G16B16A16_UNORM
+    kConvRg16s = 10,    // R16G16_SNORM (37)              -> R16G16B16A16_UNORM
+    kConvR16s = 11,     // R16_SNORM (58)                 -> R16G16B16A16_UNORM
+    kConvR11g11b10f = 12,   // R11G11B10_FLOAT (26)       -> R16G16B16A16_UNORM
+    kConvR9g9b9e5 = 13, // R9G9B9E5_SHAREDEXP (67)        -> R16G16B16A16_UNORM
+    kConvRg8 = 14,      // R8G8_UNORM (49)                -> R8G8B8A8_UNORM
+    kConvRg8s = 15,     // R8G8_SNORM (51)                -> R8G8B8A8_UNORM
+    kConvRgba8s = 16,   // R8G8B8A8_SNORM (31)            -> R8G8B8A8_UNORM
+    kConvR8s = 17,      // R8_SNORM (63)                  -> R8G8B8A8_UNORM
+    kConvA8 = 18,       // A8_UNORM (65)                  -> R8G8B8A8_UNORM
+    kConvBgra4 = 19,    // B4G4R4A4_UNORM (115)           -> R8G8B8A8_UNORM
+    kConvBgrx4 = 20,    // X4R4G4B4: B4G4R4A4_UNORM with the alpha nibble set to 0xF on load (_CopyScanline, TEXP_SCANLINE_SETALPHA)
+    kConvRg32f = 21     // R32G32_FLOAT (16)              -> R32G32B32A32_FLOAT
 };
-ITW_HD constexpr int raw_src_bytes(int src) { return src == kRawBgr8 ? 3 : src == kRawRgba16 ? 8 : src == kRawRgba32f ? 16 : 4; }
-ITW_HD constexpr int raw_plane_bytes(int src) { return src == kRawRgba16 ? 2 : src == kRawRgba32f ? 4 : 1; }
+ITW_HD constexpr int raw_src_bytes(int src)
+{
+    return src == kRawBgr8 ? 3
+         : src == kRawRgba16 || src == kConvRgba16f || src == kConvRgba16s || src == kConvRg32f ? 8
+         : src == kRawRgba32f ? 16
+         : src == kConvR16f || src == kConvR16s || src == kConvRg8 || src == kConvRg8s || src == kConvBgra4 || src == kConvBgrx4 ? 2
+         : src == kConvR8s || src == kConvA8 ? 1
+         : 4;
+}
+// bytes of one plane of the target (the layer's depth / 8)
+ITW_HD constexpr int raw_plane_bytes(int src)
+{
+    return src == kRawRgba32f || src == kConvRg32f ? 4 : src == kRawRgba16 || (src >= kConvRgba16f && src <= kConvR9g9b9e5) ? 2 : 1;
+}
+// The converted form of a loaded DXGI format, -1 for a format this path does not convert (X4R4G4B4 is chosen by its header).
+ITW_HD constexpr int conv_kind_of(unsigned dxgi)
+{
+    return dxgi == 10 ? kConvRgba16f : dxgi == 54 ? kConvR16f : dxgi == 34 ? kConvRg16f : dxgi == 13 ? kConvRgba16s
+         : dxgi == 35 ? kConvRg16 : dxgi == 37 ? kConvRg16s : dxgi == 58 ? kConvR16s : dxgi == 26 ? kConvR11g11b10f
+         : dxgi == 67 ? kConvR9g9b9e5 : dxgi == 49 ? kConvRg8 : dxgi == 51 ? kConvRg8s : dxgi == 31 ? kConvRgba8s
+         : dxgi == 63 ? kConvR8s : dxgi == 65 ? kConvA8 : dxgi == 115 ? kConvBgra4 : dxgi == 16 ? kConvRg32f : -1;
+}
+// DoReadStart's target of a converted form (:2534-2544): BitsPerColor > 16 -> 2, > 8 -> 11, else 28 (none of the forms is _SRGB); the
+// layer depth is its plane width.
+ITW_HD constexpr int conv_target_of(int src) { return raw_plane_bytes(src) == 4 ? 2 : raw_plane_bytes(src) == 2 ? 11 : 28; }
+// HasAlpha(loaded format) (DirectXTexUtil.cpp): IsAlphaAllOpaque returns early without it (DirectXTexImage.cpp:749-750)
+ITW_HD constexpr bool conv_has_alpha(int src)
+{
+    return src == kConvRgba16f || src == kConvRgba16s || src == kConvRgba8s || src == kConvA8 || src == kConvBgra4 || src == kConvBgrx4;
+}
 
 // The alpha decision of one loaded texel from the word that holds its alpha (the texel's last 32 bits): true when alpha < 0.99f.
+// Converted forms (the loaders of _LoadScanline, restated below; exact tests on the stored bits where the margins allow):
+//   R16G16B16A16_FLOAT  XMConvertHalfToFloat(a) < 0.99f, compared as a float (exponent 31 is a large finite value, never NaN)
+//   R16G16B16A16_SNORM  XMLoadShortN4 = max(-1, s * (1/32767)): 32439 -> 0.989990, 32440 -> 0.990020       -> s <= 32439
+//   R8G8B8A8_SNORM      XMLoadByteN4 = max(-1, c * (1/127)): 125 -> 0.984252, 126 -> 0.992126              -> c <= 125
+//   A8_UNORM            byte / 255.f (the hand-written loop): 252 -> 0.988235, 253 -> 0.992157           -> byte <= 252
+//   B4G4R4A4_UNORM      nibble * (1/15) (XMLoadUNibble4 * s_Scale): 14 -> 0.933333, 15 -> 1.0               -> nibble <= 14
+// A word holds one alpha (texels of 4 bytes or more), two (4444: the top nibble of each ushort) or four (A8: every byte).
 template <int kSrc>
 ITW_HD bool raw_alpha_below(u32 word)
 {
@@ -44,16 +97,158 @@ ITW_HD bool raw_alpha_below(u32 word)
         float a;
         memcpy(&a, &word, 4);
         return a < 0.99f;
+    } else if constexpr (kSrc == kConvRgba16f) {
+        return front_float_from_half(word >> 16) < 0.99f;
+    } else if constexpr (kSrc == kConvRgba16s) {
+        return (int)(short)(word >> 16) <= 32439;
+    } else if constexpr (kSrc == kConvRgba8s) {
+        return (int)(signed char)(word >> 24) <= 125;
+    } else if constexpr (kSrc == kConvA8) {
+        return (word & 0xFFu) <= 252u || ((word >> 8) & 0xFFu) <= 252u || ((word >> 16) & 0xFFu) <= 252u || (word >> 24) <= 252u;
+    } else if constexpr (kSrc == kConvBgra4) {
+        return ((word >> 12) & 0xFu) <= 14u || (word >> 28) <= 14u;
     } else {
         return (word >> 24) <= 252u;
     }
 }
 
-// The loaded texel at `p` (4-byte aligned unless kRawBgr8) as four plane values: bytes, ushorts or float bit patterns.
+ITW_HD float mul_rn(float a, float b)
+{
+#if defined(__CUDA_ARCH__)
+    return __fmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+ITW_HD float add_rn(float a, float b)
+{
+#if defined(__CUDA_ARCH__)
+    return __fadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+ITW_HD float div_rn(float a, float b)
+{
+#if defined(__CUDA_ARCH__)
+    return __fdiv_rn(a, b);
+#else
+    return a / b;
+#endif
+}
+// XMVectorSaturate (max with 0, then min with 1: a NaN becomes 0)
+ITW_HD float conv_saturate(float x)
+{
+    x = x > 0.0f ? x : 0.0f;
+    return x < 1.0f ? x : 1.0f;
+}
+// The target stores: XMStoreUShortN4 (R16G16B16A16_UNORM) and the bias + XMStoreUByteN4 of R8G8B8A8_UNORM, both ASSUMED round to
+// nearest with the half added after the product (DESIGN section 2): trunc(saturate(x) * max + 0.5).
+ITW_HD u32 conv_unorm16(float x) { return (u32)add_rn(mul_rn(conv_saturate(x), 65535.0f), 0.5f); }
+ITW_HD u32 conv_unorm8(float x) { return (u32)add_rn(mul_rn(conv_saturate(x), 255.0f), 0.5f); }
+// XMLoadShortN* / XMLoadByteN* (DirectXMath 3.06): the integer times the rounded reciprocal, clamped at -1 (-32768 and -128)
+ITW_HD float conv_snorm16(u32 bits) { const float v = mul_rn((float)(int)(short)bits, 1.0f / 32767.0f); return v > -1.0f ? v : -1.0f; }
+ITW_HD float conv_snorm8(u32 bits) { const float v = mul_rn((float)(int)(signed char)bits, 1.0f / 127.0f); return v > -1.0f ? v : -1.0f; }
+// One channel of XMLoadFloat3PK (DirectXMath 3.06): an unsigned float of a 5-bit exponent and an m-bit mantissa, exactly; exponent 31
+// is Inf / NaN.
+template <int kMant>
+ITW_HD float conv_packed_float(u32 f)
+{
+    u32 mant = f & ((1u << kMant) - 1u), exp = f >> kMant;
+    if (exp == 31u) return bits_float(0x7F800000u | (mant << (23 - kMant)));
+    if (exp == 0u) {
+        if (mant) {
+            exp = 1u;
+            do { exp--; mant <<= 1; } while (!(mant & (1u << kMant)));
+            mant &= (1u << kMant) - 1u;
+        } else {
+            exp = (u32)-112;
+        }
+    }
+    return bits_float(((exp + 112u) << 23) | (mant << (23 - kMant)));
+}
+
+// The converted texel at `p` (4-byte aligned when its texel has 4 bytes or more) as the target's planes: DirectX::Convert's _Convert
+// with filter 0 (DirectXTexConvert.cpp:4321-4400) for one texel.  _LoadScanline's case of the loaded format gives (r, g, b, a) floats
+// (absent channels 0, alpha 1); _ConvertScanline(target, loaded, 0) then applies, for these pairs, SNORM -> UNORM v * 0.5 + 0.5 on all
+// four channels, FLOAT -> UNORM saturate, or nothing (UNORM, the shared exponent, FLOAT -> FLOAT), followed by the R -> RGB splat of
+// the one-channel formats; _StoreScanline rounds into the target.  Every product and sum rounds on its own, as in the reference.
+template <int kSrc>
+ITW_HD void conv_texel(const uint8_t* p, u32 (&o)[4])
+{
+    float c[4] = {0.0f, 0.0f, 0.0f, 1.0f};
+    if constexpr (kSrc == kConvRg32f) {                  // XMLoadFloat2 and XMStoreFloat4: bit copies, (r, g, 0, 1)
+        o[0] = reinterpret_cast<const u32*>(p)[0];
+        o[1] = reinterpret_cast<const u32*>(p)[1];
+        o[2] = 0u;
+        o[3] = 0x3F800000u;
+        return;
+    } else if constexpr (kSrc == kConvRgba16f || kSrc == kConvRgba16s) {
+        const u32 lo = reinterpret_cast<const u32*>(p)[0], hi = reinterpret_cast<const u32*>(p)[1];
+        const u32 h[4] = {lo & 0xFFFFu, lo >> 16, hi & 0xFFFFu, hi >> 16};
+#pragma unroll
+        for (int k = 0; k < 4; k++) c[k] = kSrc == kConvRgba16f ? front_float_from_half(h[k]) : conv_snorm16(h[k]);
+    } else if constexpr (kSrc == kConvRg16f || kSrc == kConvRg16 || kSrc == kConvRg16s) {
+        const u32 w = *reinterpret_cast<const u32*>(p);
+#pragma unroll
+        for (int k = 0; k < 2; k++) {
+            const u32 h = (w >> (16 * k)) & 0xFFFFu;
+            c[k] = kSrc == kConvRg16f ? front_float_from_half(h) : kSrc == kConvRg16s ? conv_snorm16(h) : mul_rn((float)h, 1.0f / 65535.0f);
+        }
+    } else if constexpr (kSrc == kConvR16f) {
+        c[0] = front_float_from_half((u32)p[0] | ((u32)p[1] << 8));
+    } else if constexpr (kSrc == kConvR16s) {            // the hand-written loop: a true division, no clamp
+        c[0] = div_rn((float)(int)(short)((u32)p[0] | ((u32)p[1] << 8)), 32767.0f);
+    } else if constexpr (kSrc == kConvR11g11b10f) {
+        const u32 w = *reinterpret_cast<const u32*>(p);
+        c[0] = conv_packed_float<6>(w & 0x7FFu);
+        c[1] = conv_packed_float<6>((w >> 11) & 0x7FFu);
+        c[2] = conv_packed_float<5>(w >> 22);
+    } else if constexpr (kSrc == kConvR9g9b9e5) {        // XMLoadFloat3SE: 2^(e - 24) times each 9-bit mantissa, exactly
+        const u32 w = *reinterpret_cast<const u32*>(p);
+        const float scale = bits_float(0x33800000u + ((w >> 27) << 23));
+#pragma unroll
+        for (int k = 0; k < 3; k++) c[k] = mul_rn(scale, (float)((w >> (9 * k)) & 0x1FFu));
+    } else if constexpr (kSrc == kConvRg8) {
+        c[0] = mul_rn((float)p[0], 1.0f / 255.0f);
+        c[1] = mul_rn((float)p[1], 1.0f / 255.0f);
+    } else if constexpr (kSrc == kConvRg8s) {
+        c[0] = conv_snorm8(p[0]);
+        c[1] = conv_snorm8(p[1]);
+    } else if constexpr (kSrc == kConvRgba8s) {
+        const u32 w = *reinterpret_cast<const u32*>(p);
+#pragma unroll
+        for (int k = 0; k < 4; k++) c[k] = conv_snorm8(w >> (8 * k));
+    } else if constexpr (kSrc == kConvR8s) {             // the hand-written loop: a true division, no clamp
+        c[0] = div_rn((float)(int)(signed char)p[0], 127.0f);
+    } else if constexpr (kSrc == kConvA8) {              // (0, 0, 0, byte / 255.f)
+        c[3] = div_rn((float)p[0], 255.0f);
+    } else if constexpr (kSrc == kConvBgra4 || kSrc == kConvBgrx4) {   // XMLoadUNibble4 * (1/15), swizzled <2, 1, 0, 3>
+        const u32 w = (u32)p[0] | ((u32)p[1] << 8) | (kSrc == kConvBgrx4 ? 0xF000u : 0u);
+#pragma unroll
+        for (int k = 0; k < 4; k++) c[k] = mul_rn((float)((w >> (4 * (k == 3 ? 3 : 2 - k))) & 0xFu), 1.0f / 15.0f);
+    }
+    constexpr bool kSnorm = kSrc == kConvRgba16s || kSrc == kConvRg16s || kSrc == kConvR16s || kSrc == kConvRg8s || kSrc == kConvRgba8s ||
+                            kSrc == kConvR8s;
+    constexpr bool kFloat = kSrc == kConvRgba16f || kSrc == kConvR16f || kSrc == kConvRg16f || kSrc == kConvR11g11b10f;
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        if (kSnorm) c[k] = add_rn(mul_rn(c[k], 0.5f), 0.5f);      // XMVectorMultiplyAdd(v, g_XMOneHalf, g_XMOneHalf)
+        if (kFloat) c[k] = conv_saturate(c[k]);
+    }
+    if (kSrc == kConvR16f || kSrc == kConvR16s || kSrc == kConvR8s) c[1] = c[2] = c[0];   // R format -> RGB format
+#pragma unroll
+    for (int k = 0; k < 4; k++) o[k] = raw_plane_bytes(kSrc) == 2 ? conv_unorm16(c[k]) : conv_unorm8(c[k]);
+}
+
+// The loaded texel at `p` (4-byte aligned unless kRawBgr8 or a converted form of fewer than 4 bytes) as four plane values of the
+// target: bytes, ushorts or float bit patterns.
 template <int kSrc>
 ITW_HD void raw_load_texel(const uint8_t* p, u32 (&v)[4])
 {
-    if constexpr (kSrc == kRawBgr8) {
+    if constexpr (kSrc >= kConvRgba16f) {
+        conv_texel<kSrc>(p, v);
+    } else if constexpr (kSrc == kRawBgr8) {
         v[0] = p[2]; v[1] = p[1]; v[2] = p[0]; v[3] = 255u;
     } else if constexpr (kSrc == kRawRgba8 || kSrc == kRawRgbx8) {
         const u32 w = *reinterpret_cast<const u32*>(p);
@@ -73,21 +268,22 @@ ITW_HD void raw_load_texel(const uint8_t* p, u32 (&v)[4])
 template <int kSrc, int kPlanes>
 ITW_HD void raw_layer_texel(const u32 (&v)[4], bool force_alpha, u32 (&o)[4])
 {
-    constexpr u32 kForced = kSrc == kRawRgba16 ? 0x3C00u : kSrc == kRawRgba32f ? 0x3F800000u : 255u;
+    constexpr u32 kForced = raw_plane_bytes(kSrc) == 2 ? 0x3C00u : raw_plane_bytes(kSrc) == 4 ? 0x3F800000u : 255u;
 #pragma unroll
     for (int c = 0; c < 4; c++) o[c] = c < kPlanes ? v[c] : 0u;
     if (force_alpha) o[kPlanes - 1] = kForced;
 }
 
 #if defined(__CUDACC__)
-// The scan of `bytes` payload bytes of kSrc texels (kRawRgba8, kRawRgba16 or kRawRgba32f) at a 4-byte aligned `payload`: *flag becomes
-// 1 if any texel is not opaque.  The bytes up to the first 16-byte boundary and after the last one are read as words by the first
-// threads; the body goes in 16-byte loads, grid-stride, four loads in flight per thread.  Word j of the payload holds an alpha when
-// j % (texel words) is the texel's last word.
+// The scan of `bytes` payload bytes of kSrc texels (kRawRgba8, kRawRgba16, kRawRgba32f or a converted form with alpha) at a 4-byte
+// aligned `payload`: *flag becomes 1 if any texel is not opaque.  The bytes up to the first 16-byte boundary and after the last one are
+// read as words by the first threads; the body goes in 16-byte loads, grid-stride, four loads in flight per thread.  Word j of the
+// payload holds an alpha when j % (texel words) is the texel's last word; texels of one or two bytes put alphas in every word, and
+// their payload may end in a partial word, which one more thread reads byte by byte (its missing bytes padded with opaque ones).
 template <int kSrc>
 __global__ void __launch_bounds__(256) open_raw_alpha_kernel(const uint8_t* __restrict__ payload, long long bytes, int* __restrict__ flag)
 {
-    constexpr int kTexelWords = raw_src_bytes(kSrc) / 4;
+    constexpr int kTexelWords = raw_src_bytes(kSrc) >= 4 ? raw_src_bytes(kSrc) / 4 : 1;
     const long long id = (long long)blockIdx.x * blockDim.x + threadIdx.x, threads = (long long)gridDim.x * blockDim.x;
     const long long to16 = (long long)((16u - (unsigned)(reinterpret_cast<uintptr_t>(payload) & 15u)) & 15u);
     const long long head = to16 < bytes ? to16 : bytes;
@@ -99,6 +295,13 @@ __global__ void __launch_bounds__(256) open_raw_alpha_kernel(const uint8_t* __re
     if (id < edge) {
         const long long j = id < head / 4 ? id : tail / 4 + (id - head / 4);
         if (j % kTexelWords == kTexelWords - 1) below = raw_alpha_below<kSrc>(__ldg(words + j));
+    }
+    if constexpr (raw_src_bytes(kSrc) < 4) {
+        if (id == edge && (bytes & 3)) {
+            u32 w = 0xFFFFFFFFu;
+            for (long long b = bytes & ~3LL; b < bytes; b++) w = (w & ~(0xFFu << (8 * (b & 3)))) | ((u32)payload[b] << (8 * (b & 3)));
+            below = raw_alpha_below<kSrc>(w);
+        }
     }
     // which of a body vector's four words hold an alpha (the body starts at word head / 4)
     u32 lanes = 0;
