@@ -745,6 +745,58 @@ int itw_dds_converted_layout(itw_dds_converted_info* info, uint32_t options);
 int itw_dds_read_converted_layer(const uint8_t* file, size_t size, const itw_dds_converted_info* info, int call, void* dst,
                                  int64_t row_bytes);
 
+/* ---------------------------------------------------------------------------------------------
+ * Section 15 -- opening the other block-compressed files: the ones itw_dds_open does not serve, which DoReadStart decompresses with
+ * DirectX::Decompress (_DecompressBC, DirectXTexCompress.cpp:358-468, after its promotion of the typeless formats) as it does the
+ * formats of section 9.  Loaded format (header forms) -> decoder -> target / depth:
+ *   74 BC2_UNORM ('DX10', DXT3, DXT2), 73 BC2_TYPELESS        -> D3DXDecodeBC2                       -> 28 R8G8B8A8_UNORM, depth 8
+ *   75 BC2_UNORM_SRGB                                          -> D3DXDecodeBC2                       -> 29 R8G8B8A8_UNORM_SRGB, depth 8
+ *   77 BC3_UNORM (DXT4 only), 76 BC3_TYPELESS                  -> D3DXDecodeBC3                       -> 28, depth 8
+ *   70 BC1_TYPELESS                                            -> D3DXDecodeBC1                       -> 28, depth 8
+ *   79 BC4_TYPELESS, 82 BC5_TYPELESS                           -> BC4U / BC5U, red copied into g, b   -> 28, depth 8 (BC4)
+ *   81 BC4_SNORM ('DX10', BC4S)                                -> D3DXDecodeBC4S, v * 0.5 + 0.5, red into green and blue -> 28
+ *   84 BC5_SNORM ('DX10', BC5S)                                -> D3DXDecodeBC5S, v * 0.5 + 0.5 (blue 0 -> 128) -> 28
+ *   94 BC6H_TYPELESS                                           -> BC6H_UF16, saturated               -> 11 R16G16B16A16_UNORM, depth 16
+ *   97 BC7_TYPELESS                                            -> D3DXDecodeBC7                       -> 28, depth 8
+ * has_alpha is HasAlpha(loaded) && !IsAlphaAllOpaque() for 70, 73-77 and 97, and the plug-in's BC1 exclusion names only 71 / 72, so a
+ * BC1_TYPELESS file with punch-through texels opens with alpha.  Colours of DXT2 / DXT4 files reach the layers still premultiplied,
+ * as in the plug-in.  Refused, each with a message naming the call: the formats and forms itw_dds_open serves (use itw_dds_open),
+ * uncompressed files (use itw_dds_open_uncompressed or itw_dds_open_converted), the palettised and 3:3:2 / 4:4 expansions, volumes,
+ * arrays other than one cube map, partial cubes, truncated files and zero or oversized dimensions.  Shapes and rules are those of
+ * section 13.
+ * ------------------------------------------------------------------------------------------- */
+enum {
+    ITW_OBC_DX10 = 0,       /* 'DX10' extension header naming one of the loaded formats above except 77 (payload at 148)            */
+    ITW_OBC_DXT3 = 1,       /* FourCC DXT3 -> 74                                                                                   */
+    ITW_OBC_DXT2 = 2,       /* FourCC DXT2 -> 74 (premultiplied alpha)                                                              */
+    ITW_OBC_DXT4 = 3,       /* FourCC DXT4 -> 77 (premultiplied alpha)                                                              */
+    ITW_OBC_BC4S = 4,       /* FourCC BC4S -> 81                                                                                   */
+    ITW_OBC_BC5S = 5        /* FourCC BC5S -> 84                                                                                   */
+};
+typedef struct itw_dds_other_bc_info {
+    itw_dds_desc desc;        /* width, height, mip_levels, array_size (1 or 6), is_cubemap; dxgi_format = the loaded format       */
+    int32_t form;             /* ITW_OBC_*: the header form                                                                     */
+    uint64_t payload_offset;  /* where the payload starts in the file: 128, or 148 behind a 'DX10' header                         */
+    int32_t has_alpha;        /* loadInfo.hasAlpha: HasAlpha(loaded) && !IsAlphaAllOpaque() (alpha < 0.99f in a texel of any image);
+                                 always 0 for 79, 81, 82, 84 and 94.  Taken before the cube override                              */
+    int32_t has_mips, ask_user;   /* as in itw_dds_open_info                                                                     */
+    /* filled by itw_dds_other_bc_layout, with the meanings of itw_dds_open_info: */
+    int32_t layers, calls, planes;
+    int32_t depth;            /* 8 (bytes) or 16 (ushorts, BC6H_TYPELESS) bits per channel                                        */
+    int32_t width, height;
+    int32_t target_dxgi;      /* the target: 28, 29 or 11                                                                        */
+} itw_dds_other_bc_info;
+/* Header + the alpha check on the GPU (open_alpha_kernel over every image), as itw_dds_open.  itw_last_kernel_ms gives the scan's time
+ * (-1 when the format has no alpha).  Returns 0 on success; on failure `info` is untouched. */
+int itw_dds_open_other_bc(const uint8_t* file, size_t size, itw_dds_other_bc_info* info);
+/* The layout for the dialog's answers `options` (ITW_OPEN_*); pure arithmetic, no CUDA call.  Returns 0 on success. */
+int itw_dds_other_bc_layout(itw_dds_other_bc_info* info, uint32_t options);
+/* One DoReadContinue: the image the call reads, decompressed into the target and stored into the zeroed layer, with the rules of
+ * itw_dds_read_uncompressed_layer (cube alpha forcing, host or device operands, every argument checked before anything is enqueued).
+ * Returns 0 on success. */
+int itw_dds_read_other_bc_layer(const uint8_t* file, size_t size, const itw_dds_other_bc_info* info, int call, void* dst,
+                                int64_t row_bytes);
+
 #ifdef __cplusplus
 }
 #endif

@@ -54,7 +54,8 @@ EXPORTS = (["CompressBlocksBC1", "CompressBlocksBC3", "CompressBlocksBC4", "Comp
             "itw_decompress", "itw_preview_pixels", "itw_dds_open", "itw_dds_open_layout", "itw_dds_read_layer",
             "itw_dds_encode_layers", "itw_cube_layout", "itw_dds_encode_cube", "itw_preview_cube", "itw_preview_layers", "itw_preview_view",
             "itw_preview_uncompressed", "itw_dds_none_layout", "itw_dds_save_none", "itw_dds_open_uncompressed", "itw_dds_uncompressed_layout",
-            "itw_dds_read_uncompressed_layer", "itw_dds_open_converted", "itw_dds_converted_layout", "itw_dds_read_converted_layer"]
+            "itw_dds_read_uncompressed_layer", "itw_dds_open_converted", "itw_dds_converted_layout", "itw_dds_read_converted_layer",
+            "itw_dds_open_other_bc", "itw_dds_other_bc_layout", "itw_dds_read_other_bc_layer"]
            + ["CompressImageBC7_" + p for p in BC7_PROFILES] + ["CompressImage" + p.replace("bc6h_", "BC6H_") for p in BC6H_PROFILES]
            + ["GetProfile_" + p for p in BC7_PROFILES + BC6H_PROFILES])
 
@@ -105,6 +106,13 @@ class DdsConvertedInfo(ctypes.Structure):     # include/itw_bcn.h section 14
 
 (CONV_DX10, CONV_G16R16, CONV_A8L8, CONV_A8, CONV_A4R4G4B4, CONV_X4R4G4B4, CONV_Q16W16V16U16, CONV_R16F, CONV_G16R16F,
  CONV_A16B16G16R16F, CONV_G32R32F) = range(11)
+
+
+class DdsOtherBcInfo(ctypes.Structure):       # include/itw_bcn.h section 15: the fields of section 14
+    _fields_ = DdsConvertedInfo._fields_
+
+
+OBC_DX10, OBC_DXT3, OBC_DXT2, OBC_DXT4, OBC_BC4S, OBC_BC5S = range(6)
 
 
 class CubeOptions(ctypes.Structure):          # include/itw_bcn.h section 10
@@ -759,6 +767,54 @@ class ItwBcn(EncoderApi):
             out = np.empty((info.height, info.width, info.planes), dtype)
             if self.dds_read_converted_layer_raw(file.ctypes.data, file.size, info, call, out.ctypes.data) != 0:
                 raise RuntimeError("itw_dds_read_converted_layer failed: " + self.last_error())
+            layers.append(out)
+        return info, layers
+
+    def dds_open_other_bc_raw(self, file_ptr, size, info):
+        """itw_dds_open_other_bc on a raw address (host or device) and a DdsOtherBcInfo (or None); returns its status."""
+        f = self.lib.itw_dds_open_other_bc
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.POINTER(DdsOtherBcInfo)]
+        return f(ctypes.c_void_p(file_ptr) if file_ptr else None, size, ctypes.byref(info) if info is not None else None)
+
+    def dds_open_other_bc(self, file_ptr, size):
+        """itw_dds_open_other_bc: header + alpha check -> DdsOtherBcInfo."""
+        info = DdsOtherBcInfo()
+        if self.dds_open_other_bc_raw(file_ptr, size, info) != 0:
+            raise RuntimeError("itw_dds_open_other_bc failed: " + self.last_error())
+        return info
+
+    def dds_other_bc_layout_raw(self, info, options):
+        f = self.lib.itw_dds_other_bc_layout
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.POINTER(DdsOtherBcInfo), ctypes.c_uint32]
+        return f(ctypes.byref(info) if info is not None else None, options)
+
+    def dds_other_bc_layout(self, info, options):
+        """itw_dds_other_bc_layout: fills the layout fields of `info` (in place) for the load dialog's answers `options`."""
+        if self.dds_other_bc_layout_raw(info, options) != 0:
+            raise RuntimeError("itw_dds_other_bc_layout failed: " + self.last_error())
+        return info
+
+    def dds_read_other_bc_layer_raw(self, file_ptr, size, info, call, dst_ptr, row_bytes=0):
+        """itw_dds_read_other_bc_layer on raw addresses (host or device); returns its status."""
+        f = self.lib.itw_dds_read_other_bc_layer
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.POINTER(DdsOtherBcInfo), ctypes.c_int, ctypes.c_void_p, ctypes.c_int64]
+        return f(ctypes.c_void_p(file_ptr) if file_ptr else None, size, ctypes.byref(info) if info is not None else None, call,
+                 ctypes.c_void_p(dst_ptr) if dst_ptr else None, row_bytes)
+
+    def dds_open_other_bc_layers(self, file, options=0):
+        """The plug-in's whole open path on a host DDS blob of the block-compressed formats itw_dds_open does not serve: (info,
+        [layer arrays of height x width x planes: uint8 at depth 8, uint16 at depth 16])."""
+        file = np.ascontiguousarray(np.frombuffer(bytes(file), np.uint8))
+        info = self.dds_other_bc_layout(self.dds_open_other_bc(file.ctypes.data, file.size), options)
+        dtype = {8: np.uint8, 16: np.uint16}[info.depth]
+        layers = []
+        for call in range(info.calls):
+            out = np.empty((info.height, info.width, info.planes), dtype)
+            if self.dds_read_other_bc_layer_raw(file.ctypes.data, file.size, info, call, out.ctypes.data) != 0:
+                raise RuntimeError("itw_dds_read_other_bc_layer failed: " + self.last_error())
             layers.append(out)
         return info, layers
 

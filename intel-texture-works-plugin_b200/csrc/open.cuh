@@ -28,17 +28,86 @@
 
 namespace itw {
 
+// Float steps that must round one by one, in the reference's order, on the GPU as on the host: no contraction into a fused
+// multiply-add whatever the compiler flags.
+ITW_HD float mul_rn(float a, float b)
+{
+#if defined(__CUDA_ARCH__)
+    return __fmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+ITW_HD float add_rn(float a, float b)
+{
+#if defined(__CUDA_ARCH__)
+    return __fadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+ITW_HD float div_rn(float a, float b)
+{
+#if defined(__CUDA_ARCH__)
+    return __fdiv_rn(a, b);
+#else
+    return a / b;
+#endif
+}
+// XMVectorSaturate (max with 0, then min with 1: a NaN becomes 0)
+ITW_HD float conv_saturate(float x)
+{
+    x = x > 0.0f ? x : 0.0f;
+    return x < 1.0f ? x : 1.0f;
+}
+// The target stores: XMStoreUShortN4 (R16G16B16A16_UNORM) and the bias + XMStoreUByteN4 of R8G8B8A8_UNORM, both ASSUMED round to
+// nearest with the half added after the product (DESIGN section 2): trunc(saturate(x) * max + 0.5).
+ITW_HD u32 conv_unorm16(float x) { return (u32)add_rn(mul_rn(conv_saturate(x), 65535.0f), 0.5f); }
+ITW_HD u32 conv_unorm8(float x) { return (u32)add_rn(mul_rn(conv_saturate(x), 255.0f), 0.5f); }
+
+// ---- itw_dds_open_other_bc (include/itw_bcn.h section 15): the block-compressed files section 9 does not open ----
+// The loaded format's decoder instantiation of the kernels below, after _DecompressBC's promotion of the typeless formats
+// (DirectXTexCompress.cpp:382-392): 70 -> 71 (BC1), 73 / 74 / 75 -> 74 (BC2), 76 / 77 (DXT4) -> 77, 79 -> 80, 81 (BC4_SNORM),
+// 82 -> 83, 84 (BC5_SNORM), 94 -> 94 (BC6H_UF16 into 16-bit UNORM planes), 97 -> 98.  -1 for every other format.
+ITW_HD constexpr int obc_decoder_of(unsigned f)
+{
+    return f == 70 ? 71 : (f >= 73 && f <= 75) ? 74 : (f == 76 || f == 77) ? 77 : f == 79 ? 80 : f == 81 ? 81 : f == 82 ? 83
+         : f == 84 ? 84 : f == 94 ? 94 : f == 97 ? 98 : -1;
+}
+// DoReadStart's target (IntelPlugin.cpp:2534-2544): BitsPerColor is 16 for BC6H_TYPELESS, which the BC6H test names not, so
+// R16G16B16A16_UNORM; IsSRGB holds for BC2_UNORM_SRGB alone; every other format has at most 8 bits per colour.
+ITW_HD constexpr int obc_target_of(unsigned f) { return f == 94 ? 11 : f == 75 ? 29 : 28; }
+ITW_HD constexpr int obc_depth_of(unsigned f) { return obc_target_of(f) == 11 ? 16 : 8; }      // BitsPerColor of the target (:2591)
+// HasAlpha of the loaded format: the plug-in's BC1 exclusion (:2470-2471) names only 71 / 72, so BC1_TYPELESS counts
+ITW_HD constexpr bool obc_has_alpha(unsigned f) { return f == 70 || (f >= 73 && f <= 77) || f == 97; }
+ITW_HD constexpr int obc_block_bytes(unsigned f) { return f == 70 || f == 79 || f == 81 ? 8 : 16; }
+
 // The first alpha byte that reads as opaque (see above).
 constexpr u32 kOpaqueAlphaMin = 253u;
 
-// One block of an alpha-bearing format (77 BC3, 98 BC7; _SRGB forms decode alike): does a texel inside the image (the first `cols`
-// columns and `rows` rows of the block) have alpha below 0.99?
+// BC2's explicit alpha as a byte: D3DXDecodeBC2 (BC.cpp:794-817) gives nibble * (1/15.f), which the byte store rounds to nibble * 17.
+// The alpha scan reads the same byte: 14 -> 238, 15 -> 255, so "not opaque" (nibble * (1/15.f) < 0.99f) is byte <= 252 here too.
+ITW_HD u32 bc2_alpha_byte(u32 w0, u32 w1, int k)
+{
+    return conv_unorm8(mul_rn((float)(((k < 8 ? w0 : w1) >> (4 * (k & 7))) & 15u), 1.0f / 15.0f));
+}
+
+// One block of an alpha-bearing format (71 BC1 for BC1_TYPELESS, 74 BC2, 77 BC3, 98 BC7; _SRGB forms decode alike): does a texel
+// inside the image (the first `cols` columns and `rows` rows of the block) have alpha below 0.99?
 template <int kFormat>
 ITW_HD bool open_block_not_opaque(const u32 (&w)[4], int cols, int rows)
 {
     u32 a[16];
     if (kFormat == 77) {
         decode_alpha(a, w[0], w[1]);
+    } else if (kFormat == 74) {
+#pragma unroll
+        for (int k = 0; k < 16; k++) a[k] = bc2_alpha_byte(w[0], w[1], k);
+    } else if (kFormat == 71) {            // three-colour blocks decode index 3 to alpha 0 (punch-through), every other texel to 255
+        u32 px[16];
+        decode_bc1_colour(px, w[0], w[1], false);
+#pragma unroll
+        for (int k = 0; k < 16; k++) a[k] = px[k] >> 24;
     } else {
         u32 px[16];
         decode_bc7(px, w);                 // the reserved mode decodes to alpha 0: not opaque, as in DirectXTex
@@ -58,6 +127,75 @@ struct OpenImage {
     long long first;
     int bw, width, height;
 };
+
+// BC4_SNORM::DecodeFromIndex (BC4BC5.cpp:106-131) in its own float operations.  The mode compares the RAW signed endpoints; the values
+// read -128 as -127, so (-127, -128) runs the eight-value mode with two equal endpoints.
+ITW_HD float bc4s_float(int r0, int r1, u32 q)
+{
+    const float f0 = div_rn((float)(r0 == -128 ? -127 : r0), 127.0f), f1 = div_rn((float)(r1 == -128 ? -127 : r1), 127.0f);
+    if (q == 0u) return f0;
+    if (q == 1u) return f1;
+    if (r0 > r1) {
+        q -= 1u;
+        return div_rn(add_rn(mul_rn(f0, (float)(7u - q)), mul_rn(f1, (float)q)), 7.0f);
+    }
+    if (q == 6u) return -1.0f;
+    if (q == 7u) return 1.0f;
+    q -= 1u;
+    return div_rn(add_rn(mul_rn(f0, (float)(5u - q)), mul_rn(f1, (float)q)), 5.0f);
+}
+// _ConvertScanline's SNORM -> UNORM (DirectXTexConvert.cpp:3331-3342: XMVectorMultiplyAdd(v, 0.5, 0.5), a product and a sum) and the
+// R8G8B8A8_UNORM store
+ITW_HD u32 snorm_unorm8(float v) { return conv_unorm8(add_rn(mul_rn(v, 0.5f), 0.5f)); }
+// one BC4_SNORM channel block -> 16 bytes of the target (the eight palette bytes are computed once)
+ITW_HD void bc4s_unorm8(u32 (&val)[16], u32 w0, u32 w1)
+{
+    const int r0 = (int)(signed char)(w0 & 255u), r1 = (int)(signed char)((w0 >> 8) & 255u);
+    const unsigned long long idx = ((unsigned long long)w1 << 16) | (w0 >> 16);
+    unsigned long long pal = 0ull;
+#pragma unroll
+    for (u32 q = 0; q < 8; q++) pal |= (unsigned long long)snorm_unorm8(bc4s_float(r0, r1, q)) << (8 * q);
+#pragma unroll
+    for (int k = 0; k < 16; k++) val[k] = (u32)(pal >> (8 * ((u32)(idx >> (3 * k)) & 7u))) & 255u;
+}
+
+// One block -> 16 RGBA8 texels of R8G8B8A8_UNORM[_SRGB]: what Decompress stores for the 8-bit decoders of the open paths.
+//   74 BC2        D3DXDecodeBC2: the colour half in four-colour mode (DecodeBC1(..., false), as BC3's), the explicit alpha
+//   81 BC4_SNORM  (r, 0, 0, 1) -> SNORM -> UNORM on all four channels -> the R -> RGB copy (:3445-3457): (r', r', r', 255)
+//   84 BC5_SNORM  (r, g, 0, 1) -> SNORM -> UNORM: blue 0 becomes 0.5 (byte 128), alpha 1 stays 1
+//   the rest      display.cuh's plain decode
+template <int kFormat>
+ITW_HD void open_block_rgba8(u32 (&px)[16], const u32 (&w)[4])
+{
+    if constexpr (kFormat == 74) {
+        decode_bc1_colour(px, w[2], w[3], true);
+#pragma unroll
+        for (int k = 0; k < 16; k++) px[k] = (px[k] & 0x00FFFFFFu) | (bc2_alpha_byte(w[0], w[1], k) << 24);
+    } else if constexpr (kFormat == 81) {
+        u32 r[16];
+        bc4s_unorm8(r, w[0], w[1]);
+#pragma unroll
+        for (int k = 0; k < 16; k++) px[k] = r[k] * 0x010101u | (snorm_unorm8(1.0f) << 24);
+    } else if constexpr (kFormat == 84) {
+        u32 r[16], g[16];
+        bc4s_unorm8(r, w[0], w[1]);
+        bc4s_unorm8(g, w[2], w[3]);
+#pragma unroll
+        for (int k = 0; k < 16; k++) px[k] = r[k] | (g[k] << 8) | (snorm_unorm8(0.0f) << 16) | (snorm_unorm8(1.0f) << 24);
+    } else {
+        display_block_rgba8<kFormat, kDisplayPlain>(px, w);
+    }
+}
+// BC6H_TYPELESS (decoder 94) -> R16G16B16A16_UNORM: D3DXDecodeBC6HU's floats (display_block_f32<95>), FLOAT -> UNORM saturate and the
+// XMStoreUShortN4 store, per channel; px[k][c] is the 16-bit value.
+ITW_HD void open_block_unorm16(u32 (&px)[16][4], const u32 (&w)[4])
+{
+    display_block_f32<95>(px, w);
+#pragma unroll
+    for (int k = 0; k < 16; k++)
+#pragma unroll
+        for (int c = 0; c < 4; c++) px[k][c] = conv_unorm16(bits_float(px[k][c]));
+}
 
 #if defined(__CUDACC__)
 // The row-staged store shared by the open path's layer kernels.  A warp writes one stretch of a layer row: lane k supplies the k-th
@@ -113,8 +251,11 @@ __global__ void __launch_bounds__(256) open_alpha_kernel(const uint8_t* __restri
         const OpenImage im = images[lo];
         const int local = (int)(id - im.first), by = local / im.bw, bx = local - by * im.bw;
         u32 w[4];
-        if (kFormat == 77) {                                    // the alpha half of a BC3 block is its first 8 bytes
+        if (kFormat == 77 || kFormat == 74) {                   // the alpha half of a BC3 / BC2 block is its first 8 bytes
             const uint2 v = __ldg(reinterpret_cast<const uint2*>(payload) + 2 * id);
+            w[0] = v.x; w[1] = v.y; w[2] = w[3] = 0u;
+        } else if (kFormat == 71) {                             // 8-byte BC1 blocks
+            const uint2 v = __ldg(reinterpret_cast<const uint2*>(payload) + id);
             w[0] = v.x; w[1] = v.y; w[2] = w[3] = 0u;
         } else {
             const uint4 v = __ldg(reinterpret_cast<const uint4*>(payload) + id);
@@ -125,16 +266,17 @@ __global__ void __launch_bounds__(256) open_alpha_kernel(const uint8_t* __restri
     if (__any_sync(0xFFFFFFFFu, below) && (threadIdx.x & 31) == 0) *flag = 1;
 }
 
-// One layer: `dst` holds `height` rows of `width` texels of kPlanes channels (bytes for the LDR decoders 71/77/80/83/98, floats for
-// BC6H 95/96), rows `row_bytes` apart; dst and row_bytes are 16-byte aligned.  The image (iw x ih texels, blocks in raster order
-// in `blocks`) lands in the top-left corner.  force_alpha: the last plane of every image texel is 255 / 1.0f.
+// One layer: `dst` holds `height` rows of `width` texels of kPlanes channels (bytes for the LDR decoders 71/74/77/80/81/83/84/98,
+// floats for BC6H 95/96, ushorts for BC6H_TYPELESS 94), rows `row_bytes` apart; dst and row_bytes are 16-byte aligned.  The image
+// (iw x ih texels, blocks in raster order in `blocks`) lands in the top-left corner.  force_alpha: the last plane of every image texel
+// is 255 / 1.0f (0x3C00 at 16 bits, open_raw.cuh's rule; no 16-bit format here has alpha).
 template <int kFormat, int kPlanes>
 __global__ void __launch_bounds__(256, 2) open_layer_kernel(const uint8_t* __restrict__ blocks, int iw, int ih, uint8_t* __restrict__ dst,
                                                          int width, int height, long long row_bytes, bool force_alpha)
 {
-    constexpr bool kHdr = kFormat == 95 || kFormat == 96;
-    constexpr int kTexel = kPlanes * (kHdr ? 4 : 1);            // bytes per layer texel
-    constexpr int kTileRow = 4 * kTexel;                        // bytes of one tile's row: 12, 16, 48 or 64
+    constexpr bool kHdr = kFormat == 95 || kFormat == 96, k16 = kFormat == 94;
+    constexpr int kTexel = kPlanes * (kHdr ? 4 : k16 ? 2 : 1);  // bytes per layer texel
+    constexpr int kTileRow = 4 * kTexel;                        // bytes of one tile's row: 12, 16, 24, 32, 48 or 64
     constexpr int kWords = kTileRow / 4;
     __shared__ uint4 stage[8][staged_row_slots(kTileRow)];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -147,7 +289,7 @@ __global__ void __launch_bounds__(256, 2) open_layer_kernel(const uint8_t* __res
     uint4 v = make_uint4(0u, 0u, 0u, 0u);
     if (in_image) {
         const long long id = (long long)ty * ibw + tx;
-        if (kFormat == 71 || kFormat == 80) {
+        if (kFormat == 71 || kFormat == 80 || kFormat == 81) {
             const uint2 h = __ldg(reinterpret_cast<const uint2*>(blocks) + id);
             v.x = h.x; v.y = h.y;
         } else {
@@ -155,11 +297,13 @@ __global__ void __launch_bounds__(256, 2) open_layer_kernel(const uint8_t* __res
         }
     }
     const u32 w[4] = {v.x, v.y, v.z, v.w};
-    // the tile's texels: four float bit patterns per texel (BC6H) or one RGBA8 word; warps wholly outside the image skip the decode
+    // the tile's texels: four float bit patterns (BC6H) or ushorts (BC6H_TYPELESS) per texel, or one RGBA8 word; warps wholly outside
+    // the image skip the decode
     u32 pf[16][4], p8[16];
     if (__any_sync(0xFFFFFFFFu, in_image)) {
         if constexpr (kHdr) display_block_f32<kFormat>(pf, w);
-        else display_block_rgba8<kFormat, kDisplayPlain>(p8, w);
+        else if constexpr (k16) open_block_unorm16(pf, w);
+        else open_block_rgba8<kFormat>(p8, w);
     }
     const int cols = in_image ? min(4, iw - 4 * tx) : 0;        // texels of this tile that belong to the image
     const int span = min(128, width - 128 * chunk) * kTexel;    // bytes of the warp's part of a layer row
@@ -179,6 +323,18 @@ __global__ void __launch_bounds__(256, 2) open_layer_kernel(const uint8_t* __res
                     u32 v = (row_in && x < cols) ? pf[4 * y + x][c] : 0u;
                     if (c == kPlanes - 1 && force_alpha && row_in && x < cols) v = 0x3F800000u;
                     t[kPlanes * x + c] = v;
+                }
+        } else if constexpr (k16) {                             // ushort j of the piece is plane j % kPlanes of texel j / kPlanes
+#pragma unroll
+            for (int i = 0; i < kWords; i++) t[i] = 0u;
+#pragma unroll
+            for (int x = 0; x < 4; x++)
+#pragma unroll
+                for (int c = 0; c < kPlanes; c++) {
+                    u32 v = (row_in && x < cols) ? pf[4 * y + x][c] : 0u;
+                    if (c == kPlanes - 1 && force_alpha && row_in && x < cols) v = 0x3C00u;
+                    const int j = kPlanes * x + c;
+                    t[j >> 1] |= v << (16 * (j & 1));
                 }
         } else {
             u32 q[4];

@@ -112,40 +112,7 @@ ITW_HD bool raw_alpha_below(u32 word)
     }
 }
 
-ITW_HD float mul_rn(float a, float b)
-{
-#if defined(__CUDA_ARCH__)
-    return __fmul_rn(a, b);
-#else
-    return a * b;
-#endif
-}
-ITW_HD float add_rn(float a, float b)
-{
-#if defined(__CUDA_ARCH__)
-    return __fadd_rn(a, b);
-#else
-    return a + b;
-#endif
-}
-ITW_HD float div_rn(float a, float b)
-{
-#if defined(__CUDA_ARCH__)
-    return __fdiv_rn(a, b);
-#else
-    return a / b;
-#endif
-}
-// XMVectorSaturate (max with 0, then min with 1: a NaN becomes 0)
-ITW_HD float conv_saturate(float x)
-{
-    x = x > 0.0f ? x : 0.0f;
-    return x < 1.0f ? x : 1.0f;
-}
-// The target stores: XMStoreUShortN4 (R16G16B16A16_UNORM) and the bias + XMStoreUByteN4 of R8G8B8A8_UNORM, both ASSUMED round to
-// nearest with the half added after the product (DESIGN section 2): trunc(saturate(x) * max + 0.5).
-ITW_HD u32 conv_unorm16(float x) { return (u32)add_rn(mul_rn(conv_saturate(x), 65535.0f), 0.5f); }
-ITW_HD u32 conv_unorm8(float x) { return (u32)add_rn(mul_rn(conv_saturate(x), 255.0f), 0.5f); }
+// mul_rn / add_rn / div_rn, conv_saturate and the target stores conv_unorm16 / conv_unorm8 are open.cuh's.
 // XMLoadShortN* / XMLoadByteN* (DirectXMath 3.06): the integer times the rounded reciprocal, clamped at -1 (-32768 and -128)
 ITW_HD float conv_snorm16(u32 bits) { const float v = mul_rn((float)(int)(short)bits, 1.0f / 32767.0f); return v > -1.0f ? v : -1.0f; }
 ITW_HD float conv_snorm8(u32 bits) { const float v = mul_rn((float)(int)(signed char)bits, 1.0f / 127.0f); return v > -1.0f ? v : -1.0f; }
