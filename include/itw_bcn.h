@@ -797,6 +797,54 @@ int itw_dds_other_bc_layout(itw_dds_other_bc_info* info, uint32_t options);
 int itw_dds_read_other_bc_layer(const uint8_t* file, size_t size, const itw_dds_other_bc_info* info, int call, void* dst,
                                 int64_t row_bytes);
 
+/* ---------------------------------------------------------------------------------------------
+ * Section 16 -- opening palettised and legacy-expanded files: the D3D9-era pixel formats that LoadFromDDSMemory (DDS_FLAGS_NONE)
+ * expands while it loads (CONV_FLAGS_EXPAND, _LegacyExpandScanline, DirectXTexDDS.cpp:726-1018).  Header form -> loaded format ->
+ * target / depth:
+ *   P8        (DDS_PAL8, 8 bits)                 -> 28 R8G8B8A8_UNORM: the palette entry of the index        -> 28, depth 8
+ *   A8P8      (DDS_PAL8, 16 bits)                -> 28: the entry of the low byte, its alpha OR'd with the high byte -> 28
+ *   A8R3G3B2  (RGB, 16 bits, e0 / 1c / 03 / ff00) -> 28: each 3- / 2-bit field bit-replicated, alpha the high byte -> 28
+ *   A4L4      (LUMINANCE, 8 bits, 0f / - / - / f0) -> 115 B4G4R4A4_UNORM (l | l << 4 | l << 8 | a << 12), then DirectX::Convert's
+ *                                                   non-WIC _Convert into 28, as section 14 converts A4R4G4B4           -> 28
+ * A palettised file holds its 256 palette words (R, G, B, and a fourth byte that is the alpha: D3D9's peFlags) between the header
+ * and the payload, so its payload starts at 1152.  A P8 file whose palette has 0 in that byte opens with transparent layers, as in
+ * the plug-in.  has_alpha is IsAlphaAllOpaque on the loaded format over every texel of every image; a palette entry no texel uses
+ * never counts.  Refused, each with a message naming the call: R3G3B2 (it loads as B5G6R5_UNORM, which Convert hands to WIC),
+ * the files the calls of sections 9, 13, 14 and 15 serve (the message names the call), 'DX10' headers naming 113 (P8) or 114 (A8P8),
+ * which LoadFromDDSMemory itself refuses, every other 'DX10' header, files that end inside the palette, truncated payloads, volumes,
+ * arrays, partial cubes and zero or oversized dimensions.  Shapes and rules are those of section 13.
+ * ------------------------------------------------------------------------------------------- */
+enum {
+    ITW_EXP_P8 = 0,           /* DDS_PAL8, 8 bits -> 28 (palette at 128, payload at 1152)                                         */
+    ITW_EXP_A8P8 = 1,         /* DDS_PAL8, 16 bits -> 28 (palette at 128, payload at 1152)                                        */
+    ITW_EXP_A8R3G3B2 = 2,     /* DDS_RGB, 16 bits, masks e0 / 1c / 03 / ff00 -> 28                                                */
+    ITW_EXP_A4L4 = 3          /* DDS_LUMINANCE, 8 bits, masks 0f / 0 / 0 / f0 -> 115                                              */
+};
+typedef struct itw_dds_expanded_info {
+    itw_dds_desc desc;        /* width, height, mip_levels, array_size (1 or 6), is_cubemap; dxgi_format = the loaded format:
+                                 28, or 115 for A4L4                                                                              */
+    int32_t form;             /* ITW_EXP_*: the header form                                                                     */
+    uint64_t payload_offset;  /* where the payload starts in the file: 1152 behind a palette, else 128                            */
+    int32_t has_alpha;        /* loadInfo.hasAlpha: !IsAlphaAllOpaque() of the loaded texels (alpha < 0.99f in a texel of any
+                                 image).  Taken before the cube override                                                        */
+    int32_t has_mips, ask_user;   /* as in itw_dds_open_info                                                                     */
+    /* filled by itw_dds_expanded_layout, with the meanings of itw_dds_open_info: */
+    int32_t layers, calls, planes;
+    int32_t depth;            /* 8: bytes                                                                                        */
+    int32_t width, height;
+    int32_t target_dxgi;      /* the target: 28                                                                                  */
+} itw_dds_expanded_info;
+/* Header + the alpha check on the GPU, as itw_dds_open_uncompressed; the palette reaches the scan by value.  itw_last_kernel_ms gives
+ * the scan's time.  Returns 0 on success; on failure `info` is untouched. */
+int itw_dds_open_expanded(const uint8_t* file, size_t size, itw_dds_expanded_info* info);
+/* The layout for the dialog's answers `options` (ITW_OPEN_*); pure arithmetic, no CUDA call.  Returns 0 on success. */
+int itw_dds_expanded_layout(itw_dds_expanded_info* info, uint32_t options);
+/* One DoReadContinue: the image the call reads, expanded (and for A4L4 converted) texel by texel into the target and stored into the
+ * zeroed layer, with the rules of itw_dds_read_uncompressed_layer (cube alpha forcing, host or device operands, every argument checked
+ * before anything is enqueued).  Returns 0 on success. */
+int itw_dds_read_expanded_layer(const uint8_t* file, size_t size, const itw_dds_expanded_info* info, int call, void* dst,
+                                int64_t row_bytes);
+
 #ifdef __cplusplus
 }
 #endif

@@ -55,7 +55,8 @@ EXPORTS = (["CompressBlocksBC1", "CompressBlocksBC3", "CompressBlocksBC4", "Comp
             "itw_dds_encode_layers", "itw_cube_layout", "itw_dds_encode_cube", "itw_preview_cube", "itw_preview_layers", "itw_preview_view",
             "itw_preview_uncompressed", "itw_dds_none_layout", "itw_dds_save_none", "itw_dds_open_uncompressed", "itw_dds_uncompressed_layout",
             "itw_dds_read_uncompressed_layer", "itw_dds_open_converted", "itw_dds_converted_layout", "itw_dds_read_converted_layer",
-            "itw_dds_open_other_bc", "itw_dds_other_bc_layout", "itw_dds_read_other_bc_layer"]
+            "itw_dds_open_other_bc", "itw_dds_other_bc_layout", "itw_dds_read_other_bc_layer", "itw_dds_open_expanded",
+            "itw_dds_expanded_layout", "itw_dds_read_expanded_layer"]
            + ["CompressImageBC7_" + p for p in BC7_PROFILES] + ["CompressImage" + p.replace("bc6h_", "BC6H_") for p in BC6H_PROFILES]
            + ["GetProfile_" + p for p in BC7_PROFILES + BC6H_PROFILES])
 
@@ -113,6 +114,13 @@ class DdsOtherBcInfo(ctypes.Structure):       # include/itw_bcn.h section 15: th
 
 
 OBC_DX10, OBC_DXT3, OBC_DXT2, OBC_DXT4, OBC_BC4S, OBC_BC5S = range(6)
+
+
+class DdsExpandedInfo(ctypes.Structure):      # include/itw_bcn.h section 16: the fields of section 14
+    _fields_ = DdsConvertedInfo._fields_
+
+
+EXP_P8, EXP_A8P8, EXP_A8R3G3B2, EXP_A4L4 = range(4)
 
 
 class CubeOptions(ctypes.Structure):          # include/itw_bcn.h section 10
@@ -815,6 +823,53 @@ class ItwBcn(EncoderApi):
             out = np.empty((info.height, info.width, info.planes), dtype)
             if self.dds_read_other_bc_layer_raw(file.ctypes.data, file.size, info, call, out.ctypes.data) != 0:
                 raise RuntimeError("itw_dds_read_other_bc_layer failed: " + self.last_error())
+            layers.append(out)
+        return info, layers
+
+    def dds_open_expanded_raw(self, file_ptr, size, info):
+        """itw_dds_open_expanded on a raw address (host or device) and a DdsExpandedInfo (or None); returns its status."""
+        f = self.lib.itw_dds_open_expanded
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.POINTER(DdsExpandedInfo)]
+        return f(ctypes.c_void_p(file_ptr) if file_ptr else None, size, ctypes.byref(info) if info is not None else None)
+
+    def dds_open_expanded(self, file_ptr, size):
+        """itw_dds_open_expanded: header + alpha check -> DdsExpandedInfo."""
+        info = DdsExpandedInfo()
+        if self.dds_open_expanded_raw(file_ptr, size, info) != 0:
+            raise RuntimeError("itw_dds_open_expanded failed: " + self.last_error())
+        return info
+
+    def dds_expanded_layout_raw(self, info, options):
+        f = self.lib.itw_dds_expanded_layout
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.POINTER(DdsExpandedInfo), ctypes.c_uint32]
+        return f(ctypes.byref(info) if info is not None else None, options)
+
+    def dds_expanded_layout(self, info, options):
+        """itw_dds_expanded_layout: fills the layout fields of `info` (in place) for the load dialog's answers `options`."""
+        if self.dds_expanded_layout_raw(info, options) != 0:
+            raise RuntimeError("itw_dds_expanded_layout failed: " + self.last_error())
+        return info
+
+    def dds_read_expanded_layer_raw(self, file_ptr, size, info, call, dst_ptr, row_bytes=0):
+        """itw_dds_read_expanded_layer on raw addresses (host or device); returns its status."""
+        f = self.lib.itw_dds_read_expanded_layer
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.POINTER(DdsExpandedInfo), ctypes.c_int, ctypes.c_void_p, ctypes.c_int64]
+        return f(ctypes.c_void_p(file_ptr) if file_ptr else None, size, ctypes.byref(info) if info is not None else None, call,
+                 ctypes.c_void_p(dst_ptr) if dst_ptr else None, row_bytes)
+
+    def dds_open_expanded_layers(self, file, options=0):
+        """The plug-in's whole open path on a host P8 / A8P8 / A8R3G3B2 / A4L4 DDS blob: (info, [uint8 layer arrays of height x
+        width x planes])."""
+        file = np.ascontiguousarray(np.frombuffer(bytes(file), np.uint8))
+        info = self.dds_expanded_layout(self.dds_open_expanded(file.ctypes.data, file.size), options)
+        layers = []
+        for call in range(info.calls):
+            out = np.empty((info.height, info.width, info.planes), np.uint8)
+            if self.dds_read_expanded_layer_raw(file.ctypes.data, file.size, info, call, out.ctypes.data) != 0:
+                raise RuntimeError("itw_dds_read_expanded_layer failed: " + self.last_error())
             layers.append(out)
         return info, layers
 

@@ -48,15 +48,21 @@ enum RawSource : int {
     kConvA8 = 18,       // A8_UNORM (65)                  -> R8G8B8A8_UNORM
     kConvBgra4 = 19,    // B4G4R4A4_UNORM (115)           -> R8G8B8A8_UNORM
     kConvBgrx4 = 20,    // X4R4G4B4: B4G4R4A4_UNORM with the alpha nibble set to 0xF on load (_CopyScanline, TEXP_SCANLINE_SETALPHA)
-    kConvRg32f = 21     // R32G32_FLOAT (16)              -> R32G32B32A32_FLOAT
+    kConvRg32f = 21,    // R32G32_FLOAT (16)              -> R32G32B32A32_FLOAT
+    // The expanded forms (itw_open_exp.inc): LoadFromDDSMemory's _LegacyExpandScanline (DirectXTexDDS.cpp:726-1018) on load
+    kExpA4l4 = 22,      // A4L4 (8 bpp): the 4:4 expansion into B4G4R4A4_UNORM (115), then kConvBgra4's _Convert -> R8G8B8A8_UNORM
+    kExpA8r3g3b2 = 23,  // A8R3G3B2 (16 bpp): 3:3:2 bit replication into R8G8B8A8_UNORM, alpha the high byte
+    kExpP8 = 24,        // P8 (8 bpp): the palette entry of the index, as R8G8B8A8_UNORM
+    kExpA8p8 = 25       // A8P8 (16 bpp): the palette entry of the low byte, the high byte OR'd into its alpha
 };
 ITW_HD constexpr int raw_src_bytes(int src)
 {
     return src == kRawBgr8 ? 3
          : src == kRawRgba16 || src == kConvRgba16f || src == kConvRgba16s || src == kConvRg32f ? 8
          : src == kRawRgba32f ? 16
-         : src == kConvR16f || src == kConvR16s || src == kConvRg8 || src == kConvRg8s || src == kConvBgra4 || src == kConvBgrx4 ? 2
-         : src == kConvR8s || src == kConvA8 ? 1
+         : src == kConvR16f || src == kConvR16s || src == kConvRg8 || src == kConvRg8s || src == kConvBgra4 || src == kConvBgrx4 ||
+           src == kExpA8r3g3b2 || src == kExpA8p8 ? 2
+         : src == kConvR8s || src == kConvA8 || src == kExpA4l4 || src == kExpP8 ? 1
          : 4;
 }
 // bytes of one plane of the target (the layer's depth / 8)
@@ -80,6 +86,13 @@ ITW_HD constexpr bool conv_has_alpha(int src)
 {
     return src == kConvRgba16f || src == kConvRgba16s || src == kConvRgba8s || src == kConvA8 || src == kConvBgra4 || src == kConvBgrx4;
 }
+
+// The expanded header forms (ITW_EXP_P8, _A8P8, _A8R3G3B2, _A4L4 = 0..3 of itw_bcn.h section 16): the format LoadFromDDSMemory loads
+// (g_LegacyDDSMap, DirectXTexDDS.cpp:84-125) and the texel form.  DoReadStart's target is 28 and the depth 8 for all four: A4L4's
+// 115 goes through the non-WIC _Convert (as A4R4G4B4 does in section 14), the others are loaded as the target.
+ITW_HD constexpr unsigned exp_loaded_of(int form) { return form == 3 ? 115u : 28u; }
+ITW_HD constexpr int exp_kind_of(int form) { return form == 0 ? kExpP8 : form == 1 ? kExpA8p8 : form == 2 ? kExpA8r3g3b2 : kExpA4l4; }
+ITW_HD constexpr bool exp_has_palette(int form) { return form == 0 || form == 1; }
 
 // The alpha decision of one loaded texel from the word that holds its alpha (the texel's last 32 bits): true when alpha < 0.99f.
 // Converted forms (the loaders of _LoadScanline, restated below; exact tests on the stored bits where the margins allow):
@@ -107,9 +120,31 @@ ITW_HD bool raw_alpha_below(u32 word)
         return (word & 0xFFu) <= 252u || ((word >> 8) & 0xFFu) <= 252u || ((word >> 16) & 0xFFu) <= 252u || (word >> 24) <= 252u;
     } else if constexpr (kSrc == kConvBgra4) {
         return ((word >> 12) & 0xFu) <= 14u || (word >> 28) <= 14u;
+    } else if constexpr (kSrc == kExpA8r3g3b2) {          // the loaded alpha is the high byte of each ushort
+        return ((word >> 8) & 0xFFu) <= 252u || (word >> 24) <= 252u;
+    } else if constexpr (kSrc == kExpA4l4) {              // the loaded 4444 alpha is the high nibble of each byte
+        return ((word >> 4) & 0xFu) <= 14u || ((word >> 12) & 0xFu) <= 14u || ((word >> 20) & 0xFu) <= 14u || (word >> 28) <= 14u;
     } else {
         return (word >> 24) <= 252u;
     }
+}
+// The same for the palettised forms, whose loaded alpha is the palette entry's fourth byte (D3D9's peFlags; P8), OR'd with the
+// texel's high byte (A8P8): UNORM8 `<= 252`.  `alpha` holds the 256 entries' alpha bytes; the first `n` texels of the word are tested
+// (a payload's last word may be partial, and an index no texel holds never counts).
+template <int kSrc>
+ITW_HD bool pal_alpha_below(const uint8_t* alpha, u32 word, int n)
+{
+    bool below = false;
+    if constexpr (kSrc == kExpP8) {
+#pragma unroll
+        for (int k = 0; k < 4; k++)
+            if (k < n) below |= alpha[(word >> (8 * k)) & 0xFFu] <= 252u;
+    } else {
+#pragma unroll
+        for (int k = 0; k < 2; k++)
+            if (k < n) below |= ((u32)alpha[(word >> (16 * k)) & 0xFFu] | ((word >> (16 * k + 8)) & 0xFFu)) <= 252u;
+    }
+    return below;
 }
 
 // mul_rn / add_rn / div_rn, conv_saturate and the target stores conv_unorm16 / conv_unorm8 are open.cuh's.
@@ -133,6 +168,24 @@ ITW_HD float conv_packed_float(u32 f)
         }
     }
     return bits_float(((exp + 112u) << 23) | (mant << (23 - kMant)));
+}
+
+// _LegacyExpandScanline's rows of the expanded forms (DirectXTexDDS.cpp:807-916), per texel, without TEXP_SCANLINE_SETALPHA (none of
+// the four entries has CONV_FLAGS_NOALPHA).  A4L4 -> B4G4R4A4_UNORM: the luminance nibble into blue, green and red, alpha on top.
+ITW_HD u32 exp_a4l4_word(u32 t) { const u32 l = t & 0x0Fu; return l | (l << 4) | (l << 8) | ((t & 0xF0u) << 8); }
+// The R8G8B8A8_UNORM word of the texel at `p`: A8R3G3B2 by bit replication, P8 / A8P8 through `pal` (the file's 256 palette words).
+template <int kSrc>
+ITW_HD u32 exp_rgba8_word(const uint8_t* p, const u32* pal)
+{
+    if constexpr (kSrc == kExpP8) {
+        return pal[p[0]];
+    } else {
+        const u32 t = (u32)p[0] | ((u32)p[1] << 8);
+        if constexpr (kSrc == kExpA8p8) return pal[t & 0xFFu] | ((t & 0xFF00u) << 16);
+        else return (t & 0xE0u) | ((t & 0xE0u) >> 3) | ((t & 0xC0u) >> 6)
+                  | ((t & 0x1Cu) << 11) | ((t & 0x1Cu) << 8) | ((t & 0x18u) << 5)
+                  | ((t & 0x03u) << 22) | ((t & 0x03u) << 20) | ((t & 0x03u) << 18) | ((t & 0x03u) << 16) | ((t & 0xFF00u) << 16);
+    }
 }
 
 // The converted texel at `p` (4-byte aligned when its texel has 4 bytes or more) as the target's planes: DirectX::Convert's _Convert
@@ -190,8 +243,8 @@ ITW_HD void conv_texel(const uint8_t* p, u32 (&o)[4])
         c[0] = div_rn((float)(int)(signed char)p[0], 127.0f);
     } else if constexpr (kSrc == kConvA8) {              // (0, 0, 0, byte / 255.f)
         c[3] = div_rn((float)p[0], 255.0f);
-    } else if constexpr (kSrc == kConvBgra4 || kSrc == kConvBgrx4) {   // XMLoadUNibble4 * (1/15), swizzled <2, 1, 0, 3>
-        const u32 w = (u32)p[0] | ((u32)p[1] << 8) | (kSrc == kConvBgrx4 ? 0xF000u : 0u);
+    } else if constexpr (kSrc == kConvBgra4 || kSrc == kConvBgrx4 || kSrc == kExpA4l4) {   // XMLoadUNibble4 * (1/15), swizzled <2, 1, 0, 3>
+        const u32 w = kSrc == kExpA4l4 ? exp_a4l4_word(p[0]) : (u32)p[0] | ((u32)p[1] << 8) | (kSrc == kConvBgrx4 ? 0xF000u : 0u);
 #pragma unroll
         for (int k = 0; k < 4; k++) c[k] = mul_rn((float)((w >> (4 * (k == 3 ? 3 : 2 - k))) & 0xFu), 1.0f / 15.0f);
     }
@@ -208,12 +261,16 @@ ITW_HD void conv_texel(const uint8_t* p, u32 (&o)[4])
     for (int k = 0; k < 4; k++) o[k] = raw_plane_bytes(kSrc) == 2 ? conv_unorm16(c[k]) : conv_unorm8(c[k]);
 }
 
-// The loaded texel at `p` (4-byte aligned unless kRawBgr8 or a converted form of fewer than 4 bytes) as four plane values of the
-// target: bytes, ushorts or float bit patterns.
+// The loaded texel at `p` (4-byte aligned unless kRawBgr8 or a form of fewer than 4 bytes) as four plane values of the target: bytes,
+// ushorts or float bit patterns.  `pal`: the palette of kExpP8 / kExpA8p8.
 template <int kSrc>
-ITW_HD void raw_load_texel(const uint8_t* p, u32 (&v)[4])
+ITW_HD void raw_load_texel(const uint8_t* p, u32 (&v)[4], const u32* pal = nullptr)
 {
-    if constexpr (kSrc >= kConvRgba16f) {
+    if constexpr (kSrc >= kExpA8r3g3b2) {
+        const u32 w = exp_rgba8_word<kSrc>(p, pal);
+#pragma unroll
+        for (int c = 0; c < 4; c++) v[c] = (w >> (8 * c)) & 0xFFu;
+    } else if constexpr (kSrc >= kConvRgba16f) {
         conv_texel<kSrc>(p, v);
     } else if constexpr (kSrc == kRawBgr8) {
         v[0] = p[2]; v[1] = p[1]; v[2] = p[0]; v[3] = 255u;
@@ -242,13 +299,15 @@ ITW_HD void raw_layer_texel(const u32 (&v)[4], bool force_alpha, u32 (&o)[4])
 }
 
 #if defined(__CUDACC__)
-// The scan of `bytes` payload bytes of kSrc texels (kRawRgba8, kRawRgba16, kRawRgba32f or a converted form with alpha) at a 4-byte
+// The scan of `bytes` payload bytes of kSrc texels (kRawRgba8, kRawRgba16, kRawRgba32f, a converted form with alpha or an expanded form) at a 4-byte
 // aligned `payload`: *flag becomes 1 if any texel is not opaque.  The bytes up to the first 16-byte boundary and after the last one are
 // read as words by the first threads; the body goes in 16-byte loads, grid-stride, four loads in flight per thread.  Word j of the
 // payload holds an alpha when j % (texel words) is the texel's last word; texels of one or two bytes put alphas in every word, and
 // their payload may end in a partial word, which one more thread reads byte by byte (its missing bytes padded with opaque ones).
-template <int kSrc>
-__global__ void __launch_bounds__(256) open_raw_alpha_kernel(const uint8_t* __restrict__ payload, long long bytes, int* __restrict__ flag)
+// below(word, n): whether a texel among the first n bytes of the word is not opaque.
+template <int kSrc, class Below>
+__device__ __forceinline__ void raw_alpha_scan(const uint8_t* __restrict__ payload, long long bytes, int* __restrict__ flag,
+                                               const Below& below_of)
 {
     constexpr int kTexelWords = raw_src_bytes(kSrc) >= 4 ? raw_src_bytes(kSrc) / 4 : 1;
     const long long id = (long long)blockIdx.x * blockDim.x + threadIdx.x, threads = (long long)gridDim.x * blockDim.x;
@@ -261,13 +320,13 @@ __global__ void __launch_bounds__(256) open_raw_alpha_kernel(const uint8_t* __re
     const long long edge = head / 4 + (bytes - tail) / 4;
     if (id < edge) {
         const long long j = id < head / 4 ? id : tail / 4 + (id - head / 4);
-        if (j % kTexelWords == kTexelWords - 1) below = raw_alpha_below<kSrc>(__ldg(words + j));
+        if (j % kTexelWords == kTexelWords - 1) below = below_of(__ldg(words + j), 4);
     }
     if constexpr (raw_src_bytes(kSrc) < 4) {
         if (id == edge && (bytes & 3)) {
             u32 w = 0xFFFFFFFFu;
             for (long long b = bytes & ~3LL; b < bytes; b++) w = (w & ~(0xFFu << (8 * (b & 3)))) | ((u32)payload[b] << (8 * (b & 3)));
-            below = raw_alpha_below<kSrc>(w);
+            below = below_of(w, (int)(bytes & 3));
         }
     }
     // which of a body vector's four words hold an alpha (the body starts at word head / 4)
@@ -286,19 +345,41 @@ __global__ void __launch_bounds__(256) open_raw_alpha_kernel(const uint8_t* __re
             const u32 w[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
 #pragma unroll
             for (int k = 0; k < 4; k++)
-                if ((lanes >> k) & 1u) below |= raw_alpha_below<kSrc>(w[k]);
+                if ((lanes >> k) & 1u) below |= below_of(w[k], 4);
         }
     }
     if (__any_sync(0xFFFFFFFFu, below) && (threadIdx.x & 31) == 0) *flag = 1;
+}
+template <int kSrc>
+__global__ void __launch_bounds__(256) open_raw_alpha_kernel(const uint8_t* __restrict__ payload, long long bytes, int* __restrict__ flag)
+{
+    raw_alpha_scan<kSrc>(payload, bytes, flag, [](u32 w, int) { return raw_alpha_below<kSrc>(w); });
+}
+
+// A P8 / A8P8 file's palette, passed to the kernels by value (1 KB of kernel parameters) and copied to shared memory at CTA start, so
+// that every CTA holds it and a layer call stages only the image it reads.
+struct RawPalette {
+    u32 e[256];
+};
+// The scan of the palettised forms: open_raw_alpha_kernel's pass with the palette's alpha bytes in shared memory.  256 threads.
+template <int kSrc>
+__global__ void __launch_bounds__(256) open_pal_alpha_kernel(const uint8_t* __restrict__ payload, long long bytes, int* __restrict__ flag,
+                                                             const __grid_constant__ RawPalette pal)
+{
+    __shared__ uint8_t alpha[256];
+    alpha[threadIdx.x] = (uint8_t)(pal.e[threadIdx.x] >> 24);
+    __syncthreads();
+    raw_alpha_scan<kSrc>(payload, bytes, flag, [&](u32 w, int n) { return pal_alpha_below<kSrc>(alpha, w, n / raw_src_bytes(kSrc)); });
 }
 
 // One layer: `dst` holds `height` rows of `width` texels of kPlanes planes of raw_plane_bytes(kSrc) bytes, rows `row_bytes` apart;
 // dst and row_bytes are 16-byte aligned.  The image (iw x ih texels of raw_src_bytes(kSrc) bytes, tight rows at `src`, 4-byte aligned
 // unless kRawBgr8) lands in the top-left corner, zeros elsewhere.  A warp covers 128 texels of one layer row: each lane builds four
 // texels and store_staged_row writes the row with 16-byte stores.  force_alpha: the last plane of every image texel is forced.
+// `pal`: the palette of kExpP8 / kExpA8p8.
 template <int kSrc, int kPlanes>
-__global__ void __launch_bounds__(256) open_raw_layer_kernel(const uint8_t* __restrict__ src, int iw, int ih, uint8_t* __restrict__ dst,
-                                                             int width, int height, long long row_bytes, bool force_alpha)
+__device__ __forceinline__ void raw_layer_rows(const uint8_t* __restrict__ src, int iw, int ih, uint8_t* __restrict__ dst, int width,
+                                               int height, long long row_bytes, bool force_alpha, const u32* pal)
 {
     constexpr int kPlaneBytes = raw_plane_bytes(kSrc), kSrcBytes = raw_src_bytes(kSrc);
     constexpr int kTexel = kPlanes * kPlaneBytes;              // bytes per layer texel: 3, 4, 6, 8, 12 or 16
@@ -317,7 +398,7 @@ __global__ void __launch_bounds__(256) open_raw_layer_kernel(const uint8_t* __re
     for (int x = 0; x < 4; x++) {
         if (Y >= ih || x0 + x >= iw) break;
         u32 v[4], o[4];
-        raw_load_texel<kSrc>(srow + x * kSrcBytes, v);
+        raw_load_texel<kSrc>(srow + x * kSrcBytes, v, pal);
         raw_layer_texel<kSrc, kPlanes>(v, force_alpha, o);
 #pragma unroll
         for (int c = 0; c < kPlanes; c++) {
@@ -327,6 +408,26 @@ __global__ void __launch_bounds__(256) open_raw_layer_kernel(const uint8_t* __re
     }
     const int span = min(128, width - 128 * chunk) * kTexel;
     store_staged_row<kTileRow>(stage[warp], lane, x0 < width, t, span, dst + (long long)Y * row_bytes + (long long)chunk * 128 * kTexel);
+}
+template <int kSrc, int kPlanes>
+__global__ void __launch_bounds__(256) open_raw_layer_kernel(const uint8_t* __restrict__ src, int iw, int ih, uint8_t* __restrict__ dst,
+                                                             int width, int height, long long row_bytes, bool force_alpha)
+{
+    raw_layer_rows<kSrc, kPlanes>(src, iw, ih, dst, width, height, row_bytes, force_alpha, nullptr);
+}
+// The layer of an expanded form: for P8 / A8P8 the palette in shared memory first, then open_raw_layer_kernel's rows.  256 threads.
+// At least four CTAs per SM: ptxas's default budget for these rows (40 registers) spills the store's byte tail around its copy loop.
+template <int kSrc, int kPlanes>
+__global__ void __launch_bounds__(256, 4) open_exp_layer_kernel(const uint8_t* __restrict__ src, int iw, int ih, uint8_t* __restrict__ dst,
+                                                                int width, int height, long long row_bytes, bool force_alpha,
+                                                                const __grid_constant__ RawPalette pal)
+{
+    __shared__ u32 spal[kSrc == kExpP8 || kSrc == kExpA8p8 ? 256 : 1];
+    if constexpr (kSrc == kExpP8 || kSrc == kExpA8p8) {
+        spal[threadIdx.x] = pal.e[threadIdx.x];
+        __syncthreads();
+    }
+    raw_layer_rows<kSrc, kPlanes>(src, iw, ih, dst, width, height, row_bytes, force_alpha, spal);
 }
 #endif
 
