@@ -845,6 +845,58 @@ int itw_dds_expanded_layout(itw_dds_expanded_info* info, uint32_t options);
 int itw_dds_read_expanded_layer(const uint8_t* file, size_t size, const itw_dds_expanded_info* info, int call, void* dst,
                                 int64_t row_bytes);
 
+/* ---------------------------------------------------------------------------------------------
+ * Section 17 -- opening volume textures, 1-D textures and texture arrays: the shapes the calls of sections 9 and 13-16 refuse, in
+ * every format those calls serve.  LoadFromDDSMemory loads the whole resource (_DecodeDDSHeader's dimension branches,
+ * ScratchImage::Initialize, DirectXTexDDS.cpp:199-353, DirectXTexImage.cpp:257-301), and DoReadStart / DoReadContinue never look at
+ * the dimension, so the plug-in opens:
+ *   a volume (a legacy header with DDS_HEADER_FLAGS_VOLUME, which takes precedence over the cube caps, or 'DX10' dimension 4 with that
+ *     flag and an array size of 1): dwDepth slices at level 0, halving per level, stored level-major; up to _CountMips3D levels.
+ *     Each call reads slice 0 of its level (GetImage(mip, 0, 0)).
+ *   a 1-D texture or 1-D array ('DX10' dimension 2): height 1 (a DDS_HEIGHT header must say 1), the cube flag dropped, up to
+ *     _CountMips(w, 1) levels.
+ *   a 2-D array or cube array ('DX10' dimension 3) of more than one item, for the formats of sections 13-16 (itw_dds_open serves the
+ *     arrays of its formats).
+ * An array_size of exactly 6 is read as a cube map whatever its dimension or cube flag (IntelPlugin.cpp:2479): six layers of item i,
+ * mip 0, alpha forced when has_alpha is set.  Otherwise the calls read GetImage(call, 0, 0) when mips are layers, or the first image.
+ * has_alpha is the serving section's: HasAlpha(loaded) && !IsAlphaAllOpaque() over EVERY image (every item, level and slice), so a
+ * volume whose only translucent texels lie in slices no layer shows opens with has_alpha = 1, as in the plug-in.  Texels, targets,
+ * depths and the layer rules are the serving section's.  Refused, each with a message naming its reason: plain 2-D textures and single
+ * cube maps (the message names the call that serves them), 2-D arrays of section-9 formats (itw_dds_open), every format reason of
+ * sections 13-16 (WIC, R32G32B32_FLOAT, UINT / SINT, R3G3B2, ...), 'DX10' dimensions other than 2, 3 and 4, array size 0, a 'DX10'
+ * volume without the volume flag or with an array size above 1, a 1-D header with DDS_HEIGHT and a height other than 1, depth 0, more
+ * levels than the shape allows, an item total above 2^32 - 1, width, height or depth above 16777216, and truncated payloads.
+ * ------------------------------------------------------------------------------------------- */
+enum { ITW_STACK_BC = 9, ITW_STACK_RAW = 13, ITW_STACK_CONVERTED = 14, ITW_STACK_OTHER_BC = 15, ITW_STACK_EXPANDED = 16 };
+typedef struct itw_dds_stack_info {
+    itw_dds_desc desc;        /* width, height (1 for 1-D), mip_levels, array_size (the 'DX10' count, x6 for cube maps; 1 for a
+                                 volume), dxgi_format = the loaded format, is_cubemap                                             */
+    uint32_t dimension;       /* 1, 2 or 3 (TEX_DIMENSION_TEXTURE1D / 2D / 3D)                                                    */
+    uint32_t slices;          /* depth of level 0 of a volume, else 1                                                            */
+    int32_t section;          /* ITW_STACK_*: whose decoder / converter / expansion reads the texels                             */
+    int32_t form;             /* that section's header form (ITW_RAW_*, ITW_CONV_*, ITW_OBC_*, ITW_EXP_*; 0 for ITW_STACK_BC)     */
+    uint64_t payload_offset;  /* where the payload starts: 128, 148 behind a 'DX10' header, or 1152 behind a palette             */
+    int32_t has_alpha;        /* loadInfo.hasAlpha over every image, with the serving section's exclusions.  Taken before the cube
+                                 override                                                                                        */
+    int32_t has_mips, ask_user;   /* as in itw_dds_open_info                                                                     */
+    /* filled by itw_dds_stack_layout, with the meanings of itw_dds_open_info: */
+    int32_t layers, calls, planes;
+    int32_t depth;            /* the serving section's: 8, 16 or 32 bits per channel                                             */
+    int32_t width, height;    /* the top level (height 1 for a 1-D texture)                                                      */
+    int32_t target_dxgi;      /* the serving section's target                                                                    */
+} itw_dds_stack_info;
+/* Header + the alpha check on the GPU: the serving section's scan over every image (open_alpha_kernel over an image table of every
+ * item, level and slice; the byte-stream scans over the whole payload).  itw_last_kernel_ms gives the scan's time (-1 when the format
+ * needs no scan).  Every refusal happens before any CUDA call.  Returns 0 on success; on failure `info` is untouched. */
+int itw_dds_open_stack(const uint8_t* file, size_t size, itw_dds_stack_info* info);
+/* The layout for the dialog's answers `options` (ITW_OPEN_*); pure arithmetic, no CUDA call.  Returns 0 on success. */
+int itw_dds_stack_layout(itw_dds_stack_info* info, uint32_t options);
+/* One DoReadContinue: the image the call reads (item `call` of a six-item texture, else slice 0 of level `call` or of level 0 / mip
+ * `call` or 0 of item 0), decoded, converted or expanded by the serving section and stored into the zeroed layer, with the rules of
+ * itw_dds_read_uncompressed_layer (alpha forcing of six-item textures, 16-bit planes unscaled, host or device operands, every argument
+ * checked before anything is enqueued).  Only that image crosses the bus.  Returns 0 on success. */
+int itw_dds_read_stack_layer(const uint8_t* file, size_t size, const itw_dds_stack_info* info, int call, void* dst, int64_t row_bytes);
+
 #ifdef __cplusplus
 }
 #endif

@@ -56,7 +56,8 @@ EXPORTS = (["CompressBlocksBC1", "CompressBlocksBC3", "CompressBlocksBC4", "Comp
             "itw_preview_uncompressed", "itw_dds_none_layout", "itw_dds_save_none", "itw_dds_open_uncompressed", "itw_dds_uncompressed_layout",
             "itw_dds_read_uncompressed_layer", "itw_dds_open_converted", "itw_dds_converted_layout", "itw_dds_read_converted_layer",
             "itw_dds_open_other_bc", "itw_dds_other_bc_layout", "itw_dds_read_other_bc_layer", "itw_dds_open_expanded",
-            "itw_dds_expanded_layout", "itw_dds_read_expanded_layer"]
+            "itw_dds_expanded_layout", "itw_dds_read_expanded_layer", "itw_dds_open_stack", "itw_dds_stack_layout",
+            "itw_dds_read_stack_layer"]
            + ["CompressImageBC7_" + p for p in BC7_PROFILES] + ["CompressImage" + p.replace("bc6h_", "BC6H_") for p in BC6H_PROFILES]
            + ["GetProfile_" + p for p in BC7_PROFILES + BC6H_PROFILES])
 
@@ -121,6 +122,14 @@ class DdsExpandedInfo(ctypes.Structure):      # include/itw_bcn.h section 16: th
 
 
 EXP_P8, EXP_A8P8, EXP_A8R3G3B2, EXP_A4L4 = range(4)
+
+
+class DdsStackInfo(ctypes.Structure):         # include/itw_bcn.h section 17
+    _fields_ = [("desc", DdsDesc), ("dimension", ctypes.c_uint32), ("slices", ctypes.c_uint32), ("section", ctypes.c_int32),
+                ("form", ctypes.c_int32)] + DdsConvertedInfo._fields_[2:]
+
+
+STACK_BC, STACK_RAW, STACK_CONVERTED, STACK_OTHER_BC, STACK_EXPANDED = 9, 13, 14, 15, 16
 
 
 class CubeOptions(ctypes.Structure):          # include/itw_bcn.h section 10
@@ -870,6 +879,54 @@ class ItwBcn(EncoderApi):
             out = np.empty((info.height, info.width, info.planes), np.uint8)
             if self.dds_read_expanded_layer_raw(file.ctypes.data, file.size, info, call, out.ctypes.data) != 0:
                 raise RuntimeError("itw_dds_read_expanded_layer failed: " + self.last_error())
+            layers.append(out)
+        return info, layers
+
+    def dds_open_stack_raw(self, file_ptr, size, info):
+        """itw_dds_open_stack on a raw address (host or device) and a DdsStackInfo (or None); returns its status."""
+        f = self.lib.itw_dds_open_stack
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.POINTER(DdsStackInfo)]
+        return f(ctypes.c_void_p(file_ptr) if file_ptr else None, size, ctypes.byref(info) if info is not None else None)
+
+    def dds_open_stack(self, file_ptr, size):
+        """itw_dds_open_stack: header + alpha check -> DdsStackInfo."""
+        info = DdsStackInfo()
+        if self.dds_open_stack_raw(file_ptr, size, info) != 0:
+            raise RuntimeError("itw_dds_open_stack failed: " + self.last_error())
+        return info
+
+    def dds_stack_layout_raw(self, info, options):
+        f = self.lib.itw_dds_stack_layout
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.POINTER(DdsStackInfo), ctypes.c_uint32]
+        return f(ctypes.byref(info) if info is not None else None, options)
+
+    def dds_stack_layout(self, info, options):
+        """itw_dds_stack_layout: fills the layout fields of `info` (in place) for the load dialog's answers `options`."""
+        if self.dds_stack_layout_raw(info, options) != 0:
+            raise RuntimeError("itw_dds_stack_layout failed: " + self.last_error())
+        return info
+
+    def dds_read_stack_layer_raw(self, file_ptr, size, info, call, dst_ptr, row_bytes=0):
+        """itw_dds_read_stack_layer on raw addresses (host or device); returns its status."""
+        f = self.lib.itw_dds_read_stack_layer
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.POINTER(DdsStackInfo), ctypes.c_int, ctypes.c_void_p, ctypes.c_int64]
+        return f(ctypes.c_void_p(file_ptr) if file_ptr else None, size, ctypes.byref(info) if info is not None else None, call,
+                 ctypes.c_void_p(dst_ptr) if dst_ptr else None, row_bytes)
+
+    def dds_open_stack_layers(self, file, options=0):
+        """The plug-in's whole open path on a host volume, 1-D or array DDS blob: (info, [layer arrays of height x width x planes,
+        uint8 / uint16 / float32 by depth])."""
+        file = np.ascontiguousarray(np.frombuffer(bytes(file), np.uint8))
+        info = self.dds_stack_layout(self.dds_open_stack(file.ctypes.data, file.size), options)
+        dtype = {8: np.uint8, 16: np.uint16, 32: np.float32}[info.depth]
+        layers = []
+        for call in range(info.calls):
+            out = np.empty((info.height, info.width, info.planes), dtype)
+            if self.dds_read_stack_layer_raw(file.ctypes.data, file.size, info, call, out.ctypes.data) != 0:
+                raise RuntimeError("itw_dds_read_stack_layer failed: " + self.last_error())
             layers.append(out)
         return info, layers
 

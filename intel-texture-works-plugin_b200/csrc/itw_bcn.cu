@@ -1185,5 +1185,6 @@ int itw_bc7_phase_clocks(void* out, size_t bytes)
 #include "itw_open_conv.inc"
 #include "itw_open_other_bc.inc"
 #include "itw_open_exp.inc"
+#include "itw_open_stack.inc"
 #include "itw_cube.inc"
 #include "itw_none.inc"
