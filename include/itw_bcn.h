@@ -557,8 +557,9 @@ typedef struct itw_view {
  * (1 << mip_level), in double and truncated toward zero (an offset in (-1, 0) lands on texel 0); texels outside the source get the
  * matte bytes.  Channels (:585-624): pure R, G, B or A show grey, in a mixture alpha takes the blue slot, a channel beyond `planes`
  * shows 0.  Stores: depth 8 the byte, depth 16 FloatToByte(v / 32768.0), depth 32 FloatToByte((double)f) without gamma.
- * Not covered: the R16G16B16A16_FLOAT branch (no pane is built in that format) and `exposure` other than 1 (InitData sets 1,
- * :1889, and nothing changes it).  Either side may be host or device memory (a host source is copied whole; device operands: the
+ * The exposure is 1: the value InitData sets at every DoWriteStart (:1889, :1902), before the user moves the slider; section 18's
+ * itw_preview_view_exposed takes the slider's value.  Not covered: the R16G16B16A16_FLOAT branch (no pane is built in that
+ * format).  Either side may be host or device memory (a host source is copied whole; device operands: the
  * ordering rule of CompressBlocks*); synchronous.  Every argument is checked before anything is enqueued (null pointers, a depth,
  * planes or row_bytes the source cannot have, a non-positive view size, a zoom that is not positive and finite, mip_level outside
  * 0..30, channel bits other than ITW_VIEW_*): `dst` is then untouched.  Returns 0 on success. */
@@ -580,7 +581,8 @@ int itw_preview_view(const itw_pixel_source* source, const itw_view* view, uint8
 enum { ITW_PANE_2D = 0, ITW_PANE_CUBE_CROSS = 1, ITW_PANE_CUBE_LAYERS = 2 };
 typedef struct itw_pane_options {
     uint32_t dxgi_format;  /* the dialog's encoding: 71/72 BC1, 77/78 BC3, 80 BC4, 83 BC5, 98/99 BC7 or 28 (none, R8G8B8A8_UNORM).
-                              95 is refused (its pane goes through WIC), 96 and every other id too                               */
+                              95 is refused here (section 18's itw_preview_uncompressed_hdr builds its pane), 96 and every
+                              other id too                                                                                       */
     int32_t  texture;      /* ITW_PANE_2D (COLOR, COLOR+A, NORMAL MAP) or one of the two cube types                            */
     int32_t  mip_level;    /* cube types: the set mip level (SetMipLevel ? MipLevel : -1), -1 <= L < max(W, H).bit_length() of
                               the face; ITW_PANE_2D: must be -1                                                                  */
@@ -896,6 +898,44 @@ int itw_dds_stack_layout(itw_dds_stack_info* info, uint32_t options);
  * itw_dds_read_uncompressed_layer (alpha forcing of six-item textures, 16-bit planes unscaled, host or device operands, every argument
  * checked before anything is enqueued).  Only that image crosses the bus.  Returns 0 on success. */
 int itw_dds_read_stack_layer(const uint8_t* file, size_t size, const itw_dds_stack_info* info, int call, void* dst, int64_t row_bytes);
+
+/* ---------------------------------------------------------------------------------------------
+ * Section 18 -- the preview dialog for HDR documents: a 32-bit document saved as BC6H_UF16, the plug-in's only HDR encoding (an
+ * environment cube map, typically).  The dialog shows IDC_EXPOSURE_SLIDER for documents deeper than 16 bits (PreviewDialog.cpp:
+ * 622-635): range -1000..1000, starting at 0, and each move sets exposure = float(pow(2, pos * 0.01)) and repaints both panes
+ * (:868-887).  FetchPreviewRGB multiplies every float texel it shows by it (IntelPlugin.cpp:501, :649-651).  The original pane of
+ * BC6H_UF16 for the cube types and for mip maps from layers is GetUncompressedImageForPreview's R16G16B16A16_FLOAT scratch converted
+ * to R8G8B8A8_UNORM (:93-119, :1142-1164, :1474-1479).  DirectXTex does not hand that conversion to WIC (g_WICFormats marks the half
+ * format linear and R8G8B8A8_UNORM sRGB, so _UseWICConversion returns false), so the non-WIC _Convert runs: per channel, half ->
+ * float, saturate, UNORM8 store; alpha is converted too.  The rules of sections 11-17 hold: every argument is checked before
+ * anything is enqueued and outputs stay untouched on failure, host and device operands are accepted (device operands: the ordering
+ * rule of CompressBlocks*), the calls are synchronous, and itw_last_kernel_ms gives the time of the call's kernels.
+ * Finding, reproduced and not fixed: the original pane is clamped RGBA8, so the slider brightens the compressed pane (an
+ * R32G32B32A32_FLOAT display) but not the original pane; and the alpha shown in the blue slot of a mixed view moves with the slider.
+ * ------------------------------------------------------------------------------------------- */
+/* itw_preview_view with the dialog's exposure: FetchPreviewRGB as it runs after the slider has moved.  At depth 32 (the document or
+ * an R32G32B32A32_FLOAT pane) each shown channel is FloatToByte((double)(f * exposure)), where the product is a FLOAT product,
+ * rounded once and then widened.  The pure-alpha view of a source with more than 3 planes resets the exposure to 1 (:615-621); in a
+ * mixture that shows alpha in the blue slot, alpha is multiplied too.  Depths 8 and 16 ignore the exposure, as the plug-in does (the
+ * slider is shown at depth 32 only).  With exposure 1.0f the output equals itw_preview_view byte for byte.  Refusals: those of
+ * itw_preview_view, and an exposure that is not positive and finite.  Returns 0 on success. */
+int itw_preview_view_exposed(const itw_pixel_source* source, const itw_view* view, float exposure, uint8_t* dst);
+/* GetUncompressedImageForPreview for encoding 95 (BC6H_UF16), in the plug-in's order:
+ *   CopyDataForEncoding(DoMipMaps = false, gammaCorrect = false) through the BC6H front end (ConvertToBC6From{8,16,32}Bit) into an
+ *       R16G16B16A16_FLOAT scratch
+ *   cube types: the faces as itw_preview_cube builds them for 95, the chain to L when set, and the zeroed RGBA16F horizontal cross of
+ *       level L (4 wL x 3 hL).  A cross without L is the converted document
+ *   ITW_PANE_2D: layer 0 over the converted document (CopyLayersIntoMipMaps(..., 0, 1)) with the RGBA16F rules of
+ *       itw_dds_encode_layers
+ *   Convert(R16G16B16A16_FLOAT -> R8G8B8A8_UNORM, TEX_FILTER_DEFAULT): the non-WIC _Convert above, into `display`
+ * `o`, `document`, `layers` and `display` as for itw_preview_uncompressed; a device display that is 4-byte aligned (pointer and
+ * stride) is written in place.  `flags`: ITW_FRONT_HAS_ALPHA only.  There is no compressed size: for 95 the dialog takes it from the
+ * compressed pane (itw_preview_pixels / itw_preview_cube).  Refused (besides what itw_preview_uncompressed checks): any dxgi_format
+ * but 95 (itw_preview_uncompressed serves them), flips (BC6H has no normal-map column, :44-62), ITW_FRONT_GAMMA and
+ * ITW_FRONT_NORMALIZE, and ITW_PANE_2D without layer 0: the plug-in builds no such pane (the dialog shows the document itself, and
+ * the compressed pane comes from itw_preview_pixels).  Returns 0 on success. */
+int itw_preview_uncompressed_hdr(const itw_pane_options* o, const itw_pixel_source* document, const itw_layer_source* layers,
+                                 uint32_t flags, const rgba_surface* display);
 
 #ifdef __cplusplus
 }

@@ -57,7 +57,7 @@ EXPORTS = (["CompressBlocksBC1", "CompressBlocksBC3", "CompressBlocksBC4", "Comp
             "itw_dds_read_uncompressed_layer", "itw_dds_open_converted", "itw_dds_converted_layout", "itw_dds_read_converted_layer",
             "itw_dds_open_other_bc", "itw_dds_other_bc_layout", "itw_dds_read_other_bc_layer", "itw_dds_open_expanded",
             "itw_dds_expanded_layout", "itw_dds_read_expanded_layer", "itw_dds_open_stack", "itw_dds_stack_layout",
-            "itw_dds_read_stack_layer"]
+            "itw_dds_read_stack_layer", "itw_preview_view_exposed", "itw_preview_uncompressed_hdr"]
            + ["CompressImageBC7_" + p for p in BC7_PROFILES] + ["CompressImage" + p.replace("bc6h_", "BC6H_") for p in BC6H_PROFILES]
            + ["GetProfile_" + p for p in BC7_PROFILES + BC6H_PROFILES])
 
@@ -573,17 +573,30 @@ class ItwBcn(EncoderApi):
         return f(ctypes.byref(source) if source is not None else None, ctypes.byref(view) if view is not None else None,
                  ctypes.c_void_p(dst_ptr) if dst_ptr else None)
 
+    def preview_view_exposed(self, source, view, exposure):
+        """itw_preview_view_exposed: preview_view with the dialog's exposure (a float; the slider's float(2 ** (pos * 0.01)))."""
+        src = np.ascontiguousarray(source)
+        out = np.zeros((view.height, view.width, 3), np.uint8)
+        ps = PixelSource(src.ctypes.data, src.shape[1], src.shape[0], src.shape[2], src.itemsize * 8, 0)
+        if self.preview_view_exposed_raw(ps, view, exposure, out.ctypes.data) != 0:
+            raise RuntimeError("itw_preview_view_exposed failed: " + self.last_error())
+        return out
+
+    def preview_view_exposed_raw(self, source, view, exposure, dst_ptr):
+        """itw_preview_view_exposed on ctypes structures and a raw (host or device) address; returns its status."""
+        f = self.lib.itw_preview_view_exposed
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.POINTER(PixelSource), ctypes.POINTER(View), ctypes.c_float, ctypes.c_void_p]
+        return f(ctypes.byref(source) if source is not None else None, ctypes.byref(view) if view is not None else None, exposure,
+                 ctypes.c_void_p(dst_ptr) if dst_ptr else None)
+
     def preview_uncompressed(self, options, document, layers=None, flags=0):
         """itw_preview_uncompressed on host arrays -> (uint8 H x W x 4 pane, compressed bytes).  `document` = host numpy H x W x planes
         array; `layers` = None, or for PANE_2D one layer (channels, alpha) and for PANE_CUBE_LAYERS six entries as cube_faces takes
         them.  The pane is the document's size (2-D, or a cross without a set level) or the 4 wL x 3 hL cross of level L."""
         doc = np.ascontiguousarray(document)
         dh, dw = doc.shape[:2]
-        w, h = dw, dh
-        if options.texture != PANE_2D and not (options.texture == PANE_CUBE_CROSS and options.mip_level < 0):
-            fw, fh = (dw, dh) if options.texture == PANE_CUBE_LAYERS else ((dw // 3, dh // 4) if dw < dh else (dw // 4, dh // 3))
-            L = max(options.mip_level, 0)
-            w, h = 4 * max(1, fw >> L), 3 * max(1, fh >> L)
+        w, h = self.pane_size(options, dw, dh)
         keep = []
         arr = None
         if layers is not None:
@@ -604,6 +617,39 @@ class ItwBcn(EncoderApi):
                       ctypes.POINTER(RgbaSurface), ctypes.POINTER(ctypes.c_size_t)]
         ref = lambda x: ctypes.byref(x) if x is not None else None
         return f(ref(options), ref(document), layers, flags, ref(display), size_ref)
+
+    def preview_uncompressed_hdr(self, options, document, layers=None, flags=0):
+        """itw_preview_uncompressed_hdr on host arrays -> the uint8 H x W x 4 pane of BC6H_UF16 (options.dxgi_format 95); arguments
+        and pane size as for preview_uncompressed."""
+        doc = np.ascontiguousarray(document)
+        w, h = self.pane_size(options, doc.shape[1], doc.shape[0])
+        keep = []
+        arr = None
+        if layers is not None:
+            arr = self.cube_faces([layers] if options.texture == PANE_2D else layers, doc.dtype, keep)
+        img = np.zeros((h, w, 4), np.uint8)
+        src = PixelSource(doc.ctypes.data, doc.shape[1], doc.shape[0], doc.shape[2], doc.itemsize * 8, 0)
+        if self.preview_uncompressed_hdr_raw(options, src, arr, flags, RgbaSurface(img.ctypes.data, w, h, img.strides[0])) != 0:
+            raise RuntimeError("itw_preview_uncompressed_hdr failed: " + self.last_error())
+        return img
+
+    def preview_uncompressed_hdr_raw(self, options, document, layers, flags, display):
+        """itw_preview_uncompressed_hdr on ctypes structures (any of them may be None); returns its status."""
+        f = self.lib.itw_preview_uncompressed_hdr
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.POINTER(PaneOptions), ctypes.POINTER(PixelSource), ctypes.POINTER(LayerSource), ctypes.c_uint32,
+                      ctypes.POINTER(RgbaSurface)]
+        ref = lambda x: ctypes.byref(x) if x is not None else None
+        return f(ref(options), ref(document), layers, flags, ref(display))
+
+    @staticmethod
+    def pane_size(options, dw, dh):
+        """(width, height) of an uncompressed pane: the document's (2-D, or a cross without a set level), else the 4 wL x 3 hL cross."""
+        if options.texture == PANE_2D or (options.texture == PANE_CUBE_CROSS and options.mip_level < 0):
+            return dw, dh
+        fw, fh = (dw, dh) if options.texture == PANE_CUBE_LAYERS else ((dw // 3, dh // 4) if dw < dh else (dw // 4, dh // 3))
+        L = max(options.mip_level, 0)
+        return 4 * max(1, fw >> L), 3 * max(1, fh >> L)
 
     def none_layout(self, options, doc_width, doc_height):
         """itw_dds_none_layout: (file size, DdsDesc, level-0 width, level-0 height); size 0 (and the error text) when refused."""

@@ -83,6 +83,10 @@ ITW_HD void display_bc4_srgb_out(u32 (&val)[16], u32 w0, u32 w1)
     for (int k = 0; k < 16; k++) val[k] = (u32)(pal >> (8 * ((u32)(idx >> (3 * k)) & 7u))) & 255u;
 }
 
+// kDisplayHdrUnorm's element: half -> float (XMLoadHalf4), FLOAT -> UNORM saturate (_ConvertScanline, :3340-3350), UNORM8 store.
+// Also the whole of the non-WIC _Convert(R16G16B16A16_FLOAT -> R8G8B8A8_UNORM) of the HDR original pane, channel by channel.
+ITW_HD u32 display_hdr_unorm8(u32 half) { return mip_unorm8_store(front_float_from_half(half)); }
+
 // ---- one block -> 16 RGBA8 texels (targets 28 / 29); kFormat is the decoder (71/77/80/83/98), kRule a DisplayRule ----
 template <int kFormat, int kRule>
 ITW_HD void display_block_rgba8(u32 (&px)[16], const u32 (&w)[4])
@@ -92,8 +96,8 @@ ITW_HD void display_block_rgba8(u32 (&px)[16], const u32 (&w)[4])
         decode_bc6h<kFormat == 96>(h, w);
 #pragma unroll
         for (int k = 0; k < 16; k++)
-            px[k] = mip_unorm8_store(front_float_from_half(h[k][0] & 0xFFFFu)) | (mip_unorm8_store(front_float_from_half(h[k][0] >> 16)) << 8) |
-                    (mip_unorm8_store(front_float_from_half(h[k][1] & 0xFFFFu)) << 16) | 0xFF000000u;
+            px[k] = display_hdr_unorm8(h[k][0] & 0xFFFFu) | (display_hdr_unorm8(h[k][0] >> 16) << 8) | (display_hdr_unorm8(h[k][1] & 0xFFFFu) << 16) |
+                    0xFF000000u;
         return;
     }
     if (kFormat == 80) {                                          // R format -> RGB format (:3445-3457): red copied into green and blue
@@ -201,6 +205,18 @@ __global__ void __launch_bounds__(128) display_kernel(const uint8_t* __restrict_
             }
         }
     }
+}
+// The HDR original pane (itw_preview_uncompressed_hdr): DirectX::Convert(R16G16B16A16_FLOAT -> R8G8B8A8_UNORM, TEX_FILTER_DEFAULT)
+// of a w x h RGBA16F scratch, which takes the non-WIC _Convert (DirectXTexConvert.cpp:4321-): all four channels through
+// display_hdr_unorm8, alpha included.  Grid (ceil(w / 256), h); 8 B read and 4 B written per texel.
+__global__ void __launch_bounds__(256) hdr_unorm8_kernel(const uint8_t* __restrict__ src, long long sstride, int w, int h, uint8_t* __restrict__ dst,
+                                                         long long dstride)
+{
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+    if (x >= w || y >= h) return;
+    const uint2 t = __ldg(reinterpret_cast<const uint2*>(src + (long long)y * sstride) + x);
+    reinterpret_cast<u32*>(dst + (long long)y * dstride)[x] = display_hdr_unorm8(t.x & 0xFFFFu) | (display_hdr_unorm8(t.x >> 16) << 8) |
+                                                              (display_hdr_unorm8(t.y & 0xFFFFu) << 16) | (display_hdr_unorm8(t.y >> 16) << 24);
 }
 // Every texel of a w x h surface := one constant texel (1 word for RGBA8, 2 for RGBA16F).  The preview cross: cells without a face.
 __global__ void __launch_bounds__(256) fill_texels_kernel(uint8_t* __restrict__ ptr, int w, int h, long long stride, int words, u32 lo, u32 hi)

@@ -801,6 +801,14 @@ int launch_fill(uint8_t* dst, int w, int h, long long stride, int words, u32 lo,
     const cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : fail("fill_texels_kernel", e);
 }
+// Convert(R16G16B16A16_FLOAT -> R8G8B8A8_UNORM) of the w x h RGBA16F image at `src` into `dst` (4-byte aligned, as `dstride`).
+int launch_hdr_unorm8(const uint8_t* src, long long sstride, int w, int h, uint8_t* dst, long long dstride, cudaStream_t s)
+{
+    hdr_unorm8_kernel<<<dim3((unsigned)((w + 255) / 256), (unsigned)h), 256, 0, s>>>(src, sstride, w, h, dst, dstride);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail("hdr_unorm8_kernel", e);
+}
 // NormalizeNormalMapChain's per-texel step over the w x h surface at `p`: RGBA16F when `hdr`, else RGBA8.
 int launch_normalize(uint8_t* p, int w, int h, long long stride, bool hdr, cudaStream_t s)
 {

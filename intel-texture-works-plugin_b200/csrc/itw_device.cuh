@@ -106,6 +106,32 @@ ITW_HD float fma_rn(float a, float b, float c)
     return fmaf(a, b, c);
 #endif
 }
+// Float steps that must round one by one, in the reference's order, on the GPU as on the host: no contraction into a fused
+// multiply-add whatever the compiler flags.
+ITW_HD float mul_rn(float a, float b)
+{
+#if defined(__CUDA_ARCH__)
+    return __fmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+ITW_HD float add_rn(float a, float b)
+{
+#if defined(__CUDA_ARCH__)
+    return __fadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+ITW_HD float div_rn(float a, float b)
+{
+#if defined(__CUDA_ARCH__)
+    return __fdiv_rn(a, b);
+#else
+    return a / b;
+#endif
+}
 ITW_HD float div_by_rcp(float x, float d, float rcp_d)
 {
     const float q = x * rcp_d;

@@ -28,32 +28,6 @@
 
 namespace itw {
 
-// Float steps that must round one by one, in the reference's order, on the GPU as on the host: no contraction into a fused
-// multiply-add whatever the compiler flags.
-ITW_HD float mul_rn(float a, float b)
-{
-#if defined(__CUDA_ARCH__)
-    return __fmul_rn(a, b);
-#else
-    return a * b;
-#endif
-}
-ITW_HD float add_rn(float a, float b)
-{
-#if defined(__CUDA_ARCH__)
-    return __fadd_rn(a, b);
-#else
-    return a + b;
-#endif
-}
-ITW_HD float div_rn(float a, float b)
-{
-#if defined(__CUDA_ARCH__)
-    return __fdiv_rn(a, b);
-#else
-    return a / b;
-#endif
-}
 // XMVectorSaturate (max with 0, then min with 1: a NaN becomes 0)
 ITW_HD float conv_saturate(float x)
 {
